@@ -62,7 +62,7 @@ __device__ __forceinline__ void frames_group(const FrameArgs& a, int first_tile)
   int* next = reinterpret_cast<int*>(empty + 2);
 
   __syncthreads();  // (mixed launches: every warp is done with the previous group's table, ring and barriers)
-  load_shared_table(*st, a.table);
+  load_shared_table(*st, a.table, pass_slot_width<BW>());
   if (threadIdx.x == 0) {
     mbar_init(&full[0], 1);
     mbar_init(&full[1], 1);
@@ -222,7 +222,7 @@ template <int G, int BW, int NW>
 __global__ void __launch_bounds__(NW * 32, 1) dexr_sequences_kernel(const SeqArgs a) {
   unsigned char* const smem = dsmem;
   SharedTable* st = reinterpret_cast<SharedTable*>(smem);
-  load_shared_table(*st, a.table);
+  load_shared_table(*st, a.table, pass_slot_width<BW>());
   __syncthreads();
 
   constexpr int GPW = 32 / G;

@@ -41,7 +41,7 @@
 //   * the short run-time loops of the FK rounds / link placement stay ROLLED (`DEXR_ROLL`): the compiler otherwise unrolls
 //     them 3-4x with remainder loops for trip counts of 1-2, and the LM loop body is instruction-fetch bound;
 //   * MERGED RESIDUAL PASSES: a residual only touches the joints above its links; residuals that touch disjoint sets of lane
-//     slots (block mode: the block_width-lane windows; dense mode: 4-lane chunks) are packed into the same pass (greedy, once
+//     slots (block mode: the BW-lane windows; dense mode: 4-lane chunks) are packed into the same pass (greedy, once
 //     per CTA: SharedTable::pass_res) and every lane works on the residual of its slot, instead of all lanes walking all
 //     n_res residuals.  Allegro / LEAP vector: 1 pass instead of 4; DexPilot on a palm-fixed hand: the wrist -> tip vectors
 //     share a pass and disjoint finger pairs share passes (4 instead of 10).  Hands with wrist joints above every finger get
@@ -208,7 +208,8 @@ __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t by
 // depends on them is provably warp-uniform for the compiler (no divergence scaffolding around shuffles).
 struct Dims {
   int dof, n_var, n_fixed, n_links, n_res, loss, n_rounds, has_mimic, num_fingers, len_proj, len_s1;
-  int block_width;  // 0 = dense Hessian; 4 / 8 = the Hessian is block diagonal over aligned lane windows of this width
+  int block_width;  // the table's: 0 = dense Hessian; 4 / 8 = the Hessian is block diagonal over aligned lane windows of this
+                    // width (only Solver<16, 4> factorises block by block; every other instantiation treats it as dense)
   int trunk;        // arrow mode only: number of trunk lanes (lanes 0..trunk-1), see Solver
 };
 
@@ -231,13 +232,22 @@ struct SharedTable {
   int group_count[DEXR_MAX_LANES];
   int group_lane[DEXR_MAX_LANES][DEXR_MAX_GROUP];
   float group_mult[DEXR_MAX_LANES][DEXR_MAX_GROUP];
-  // pass_res[r][slot]: the residual the lanes of `slot` work on in pass r, -1 = none (slot = lane / block_width in block
-  // mode, lane / 4 in dense mode)
+  // pass_res[r][slot]: the residual the lanes of `slot` work on in pass r, -1 = none (slot = lane / pass_slot_width<BW>() of
+  // the Solver instantiation that reads it: BW lanes in block mode, 4 in dense mode -- also for a table with block_width 8,
+  // which runs densely because there is no <G, 8> instantiation)
   int pass_res[DEXR_MAX_RES][DEXR_MAX_LANES / 4];
   int n_pass;
 };
 
-__device__ inline void load_shared_table(SharedTable& st, const dexr_table_t* __restrict__ tb) {
+// Lanes per residual-pass slot of Solver<G, BW>: the schedule in SharedTable::pass_res must be built with the width the
+// running instantiation reads it with, not with the table's block_width.
+template <int BW>
+__host__ __device__ constexpr int pass_slot_width() { return BW > 0 ? BW : 4; }
+
+// slot_width: pass_slot_width<BW>() of the Solver instantiation that runs on this table.  The default, 4, is that width for
+// every instantiation there is (<16, 4>, <16, 0>, <32, 0>, and <32, -1>, which does not read the schedule); a table with
+// block_width 8 runs densely and gets 4-lane slots too.
+__device__ inline void load_shared_table(SharedTable& st, const dexr_table_t* __restrict__ tb, int slot_width = 4) {
   for (int i = threadIdx.x; i < DEXR_MAX_LINKS; i += blockDim.x) {
     st.link_off[i] = make_float4(tb->link_off[i][0], tb->link_off[i][1], tb->link_off[i][2],
                                  __int_as_float(tb->link_parent[i]));
@@ -274,7 +284,7 @@ __device__ inline void load_shared_table(SharedTable& st, const dexr_table_t* __
       }
       st.own_rounds = mx > DEXR_MAX_LINKS_PER_LANE ? DEXR_MAX_LINKS_PER_LANE : mx;
       {
-        const int gr = tb->block_width > 0 ? tb->block_width : 4;  // lanes per slot
+        const int gr = slot_width;  // lanes per slot
         const int nslot = DEXR_MAX_LANES / 4;
         const bool merge = !(tb->block_width == 0 && tb->has_mimic);  // mimic fold: keep one residual per pass
         for (int r = 0; r < DEXR_MAX_RES; ++r)
@@ -735,7 +745,7 @@ struct Solver {
         bool on = true;  // merged mode: false on the lanes of a slot that has no residual in this pass
         if constexpr (merged) {
           const int kq = two_halves ? 2 * kk + duo : kk;       // this half's pass
-          const int kw = ST().pass_res[kq < n_pass ? kq : 0][l / (BW > 0 ? BW : 4)];
+          const int kw = ST().pass_res[kq < n_pass ? kq : 0][l / pass_slot_width<BW>()];
           on = kq < n_pass && kw >= 0;
           k = on ? kw : 0;
         }

@@ -81,7 +81,9 @@ typedef struct dexr_table {
   int32_t len_s1;      /* dexpilot: pairs involving the first finger (thumb) */
   int32_t block_width; /* 0: dense Hessian.  4 / 8: the joints split into decoupled groups occupying aligned lane
                           windows of this width (no residual and no ancestor relation crosses a window), so the
-                          Newton system is block diagonal and all blocks are factorised side by side */
+                          Newton system is block diagonal.  4 (dof <= 16): all blocks are factorised side by side.
+                          8, or 4 with dof > 16: accepted and factorised densely (there is no solver instantiation
+                          for those widths); the result is the same minimiser */
   int32_t arrow;       /* 0: none.  1 + t: ARROW structure -- lanes 0..t-1 (t <= 8) are a trunk (free-flying base and / or
                           wrist) shared by decoupled fingers, each a contiguous run of <= 8 lanes whose first lane is an
                           ancestor of the others; every residual touches the trunk and at most one finger.  The Newton

@@ -135,7 +135,7 @@ int run_all(char* err, int errlen) {
   const int scratch_bytes = GPW * Scratch<G>::kFloats * 4;
   if (job.scratch_off + scratch_bytes > (int)sizeof(dsmem)) { snprintf(err, errlen, "emulated shared memory too small"); return -2; }
   threadIdx.x = 0; blockDim.x = 1;
-  load_shared_table(*reinterpret_cast<SharedTable*>(dsmem), job.tb);
+  load_shared_table(*reinterpret_cast<SharedTable*>(dsmem), job.tb, pass_slot_width<BW>());
   for (job.base = 0; job.base < job.B; job.base += GPW) {
     uint32_t* sc = reinterpret_cast<uint32_t*>(dsmem + job.scratch_off);
     for (int i = 0; i < scratch_bytes / 4; ++i) sc[i] = 0x7fc00000u;  // NaN poison
@@ -238,7 +238,7 @@ int run_streams(char* err, int errlen) {
   job.scratch_off = ((int)sizeof(SharedTable) + 15) / 16 * 16;
   const int scratch_bytes = GPW * Scratch<G>::kFloats * 4;
   threadIdx.x = 0; blockDim.x = 1;
-  load_shared_table(*reinterpret_cast<SharedTable*>(dsmem), job.tb);
+  load_shared_table(*reinterpret_cast<SharedTable*>(dsmem), job.tb, pass_slot_width<BW>());
   for (sjob.base = 0; sjob.base < sjob.S; sjob.base += (G == 16 && sjob.duo) ? 1 : GPW) {
     uint32_t* sc = reinterpret_cast<uint32_t*>(dsmem + job.scratch_off);
     for (int i = 0; i < scratch_bytes / 4; ++i) sc[i] = 0x7fc00000u;

@@ -66,9 +66,10 @@ def solve_frames(opt, last_qpos, keypoints=None, ref_value=None, fixed_qpos=None
     return (out, status, cost, full) if want_robot_qpos else (out, status, cost)
 
 
-def solve_sequences(seq, keypoints, state=None, defines=(), use_arrow=True, raw_hand=None, duo=False):
-    """Emulated dexr_solve_sequences for a SeqRetargeting of the host mirror: keypoints [S,T,21,3] -> filtered robot qpos
-    [S,T,dof]; `state` = dict(last_qpos, filter_state, filter_init, projected, damping) carried between calls (created if None).
+def solve_sequences(seq, keypoints, state=None, defines=(), use_arrow=True, raw_hand=None, duo=False, fixed_qpos=None):
+    """Emulated dexr_solve_sequences for a SeqRetargeting of the host mirror: keypoints [S,T,21,3] (+ fixed_qpos [S,T,n_fixed]
+    when the robot has fixed joints) -> filtered robot qpos [S,T,dof]; `state` = dict(last_qpos, filter_state, filter_init,
+    projected, damping) carried between calls (created if None).
     `duo`: the scarce-streams mode of the 16-lane solver (both half-warps on one stream, residual passes split)."""
     from dex_retargeting_b200 import _native as N
 
@@ -77,7 +78,11 @@ def solve_sequences(seq, keypoints, state=None, defines=(), use_arrow=True, raw_
     table, prm = opt.build_table(), opt.params(clip_init=True, lp_alpha=seq.low_pass_alpha, raw_hand=raw_hand)
     kp = np.ascontiguousarray(keypoints, dtype=np.float32)
     S, T = kp.shape[:2]
-    assert table.n_fixed == 0, "streams with fixed joints: not wired in the emulation helper"
+    fixed = None
+    if table.n_fixed > 0:
+        assert fixed_qpos is not None, f"robot has {table.n_fixed} fixed joints but no fixed_qpos is given"
+        fixed = np.ascontiguousarray(fixed_qpos, dtype=np.float32)
+        assert fixed.shape == (S, T, table.n_fixed), fixed.shape
     if state is None:  # SeqRetargeting.make_stream_state: mid-range warm start, filter not initialised, no projection
         state = dict(last_qpos=np.tile(seq.joint_limits.mean(1).astype(np.float32), (S, 1)),
                      filter_state=np.zeros((S, table.dof), np.float32), filter_init=np.zeros(S, np.uint8),
@@ -87,6 +92,8 @@ def solve_sequences(seq, keypoints, state=None, defines=(), use_arrow=True, raw_
     status = np.zeros((S, T), np.int32)
     io = N.DexrSequences()
     io.keypoints, io.last_qpos = kp.ctypes.data, state["last_qpos"].ctypes.data
+    if fixed is not None:
+        io.fixed_qpos = fixed.ctypes.data
     io.filter_state, io.filter_init = state["filter_state"].ctypes.data, state["filter_init"].ctypes.data
     io.projected = state["projected"].ctypes.data if state["projected"] is not None else None
     io.robot_qpos_out, io.status_out = out.ctypes.data, status.ctypes.data

@@ -185,9 +185,16 @@ def test_block_width_detection():
         assert build_product(key).optimizer.build_table().block_width == bw, key
 
 
-def _pass_schedule(t):
-    """Mirror of the greedy pass scheduler in load_shared_table (csrc/dexr_kernels.cuh, merged residual passes)."""
-    gr, nslot = (t.block_width if t.block_width > 0 else 4), 8
+def _solver_bw(t):
+    """BW of the Solver<G, BW> instantiation the library runs the table on (dexr.cu solver_kind; arrow counts as dense here:
+    it does not read the merged schedule)."""
+    return 4 if t.dof <= 16 and t.block_width == 4 else 0
+
+
+def _pass_schedule(t, bw):
+    """Mirror of the greedy pass scheduler in load_shared_table (csrc/dexr_kernels.cuh, merged residual passes), built for
+    the instantiation Solver<G, bw> that reads it: slots of pass_slot_width<bw>() lanes."""
+    gr, nslot = (bw if bw > 0 else 4), 8
     merge = not (t.block_width == 0 and t.has_mimic)
     passes, touched = [], []
     for k in range(t.n_res):
@@ -216,7 +223,7 @@ def test_merged_residual_passes_are_a_valid_schedule():
     counts = {}
     for key in sorted(configs()):
         t = build_product(key).optimizer.build_table()
-        passes, touched = _pass_schedule(t)
+        passes, touched = _pass_schedule(t, _solver_bw(t))
         assert len(passes) <= t.n_res
         for k in range(t.n_res):
             where = [(r, sl) for r, row in enumerate(passes) for sl, v in enumerate(row) if v == k]
@@ -229,6 +236,25 @@ def test_merged_residual_passes_are_a_valid_schedule():
     assert counts["teleop/leap_hand_right_dexpilot"] == 4 and counts["teleop/allegro_hand_right_dexpilot"] == 4  # 3 rounds of pairs + wrist
     assert counts["teleop/ability_hand_right"] == 5       # mimic joints: no merging
     assert counts["offline/shadow_hand_right"] == 10      # every residual touches the free-flying base
+
+
+def test_merged_residual_passes_on_synthetic_robots(tmp_path):
+    """The same schedule properties for the synthetic robots of tests/structure_cases.py, block width 8 among them: a
+    width-8 table runs on a dense instantiation, so its schedule has 4-lane slots (a residual of an 8-lane window owns
+    both slots of the window)."""
+    import structure_cases as SC
+
+    for case in SC.CASES:
+        seq, _ = SC.build(case, tmp_path)
+        t = seq.optimizer.build_table()
+        passes, touched = _pass_schedule(t, _solver_bw(t))
+        for k in range(t.n_res):
+            where = [(r, sl) for r, row in enumerate(passes) for sl, v in enumerate(row) if v == k]
+            assert len({r for r, _ in where}) == 1, (case.id, k)
+            assert sum(1 << sl for _, sl in where) == touched[k], (case.id, k)
+        if t.block_width == 8:
+            assert _solver_bw(t) == 0 and any(bin(sm).count("1") == 2 for sm in touched), case.id
+        assert len(passes) <= t.n_res, case.id
 
 
 def test_library_rejects_inconsistent_block_width():

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Dry run of the GPU parity suite on the CPU: the test functions of tests/test_gpu_{parity,golden,arrow}.py are called
+"""Dry run of the GPU parity suite on the CPU: the test functions of tests/test_gpu_{parity,golden,arrow,structures}.py are called
 unchanged while the two device entry points of the host mirror (Optimizer.retarget_batch, SeqRetargeting.retarget_sequences)
 are served by the HOST EMULATION of the solver source (tests/emu) -- for a chosen set of compile-time experiment switches.
 Inside the test modules `torch` is a proxy that maps every device to the CPU.  Not covered: the pinned-host entry, multi-GPU,
@@ -35,7 +35,8 @@ SKIP = {"test_host_buffer_entry_matches_device_entry": "pinned-host entry (dexr_
         "test_single_frame_api_matches_batch_and_oracle": "single-frame host entry",
         "test_maximum_size_robot_parity": "uses the host entry",
         "test_empty_batch_is_a_no_op": "host entry",
-        "test_carried_damping_through_every_entry_point": "host entries (the device part passes: 0.95 of the cold starts in the same minimum)"}
+        "test_carried_damping_through_every_entry_point": "host entries (the device part passes: 0.95 of the cold starts in the same minimum)",
+        "test_mixed_launch_with_structure_cases": "mixed-robot launch (dexr_solve_frames_multi)"}
 
 
 class FakeEngine:
@@ -106,7 +107,8 @@ def retarget_sequences(self, keypoints, state=None, fixed_qpos=None, out=None, s
     state = state if state is not None else self.make_stream_state(S)
     st = dict(last_qpos=_np(state.last_qpos), filter_state=_np(state.filter_state), filter_init=_np(state.filter_init),
               projected=_np(state.projected), damping=_np(state.damping))
-    got, status, _ = emu_host.solve_sequences(self, _np(keypoints), state=st, defines=DEFINES, use_arrow=use_arrow())
+    got, status, _ = emu_host.solve_sequences(self, _np(keypoints), state=st, defines=DEFINES, use_arrow=use_arrow(),
+                                              fixed_qpos=_np(fixed_qpos))
     if status_out is not None:
         status_out.copy_(real_torch.from_numpy(status))
     if out is not None:
@@ -143,10 +145,10 @@ def main():
     Optimizer.engine = lambda self: FakeEngine(self)
     SeqRetargeting.make_stream_state = make_stream_state
     SeqRetargeting.retarget_sequences = retarget_sequences
-    import test_gpu_arrow, test_gpu_golden, test_gpu_parity  # noqa: E401
+    import test_gpu_arrow, test_gpu_golden, test_gpu_parity, test_gpu_structures  # noqa: E401
 
     failed = ran = 0
-    for mod in (test_gpu_parity, test_gpu_golden, test_gpu_arrow):
+    for mod in (test_gpu_parity, test_gpu_golden, test_gpu_arrow, test_gpu_structures):
         mod.torch = TorchProxy()
         for name in [n for n in dir(mod) if n.startswith("test_")]:
             fn = getattr(mod, name)
