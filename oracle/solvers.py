@@ -96,9 +96,10 @@ def _fold(o, Hq):
     return M.T @ Hq @ M
 
 
-def _ggn_hessian(obj, x):
+def _ggn_hessian(obj, x, majoriser=False):
     """Exact Hessian of the consistent objective: loss curvature through the Jacobian + the kinematic
-    second-derivative term + the regulariser."""
+    second-derivative term + the regulariser.  `majoriser` (position loss only): beyond the quadratic
+    zone a coordinate contributes the curvature 1/|d| of the Huber majoriser instead of the exact 0."""
     o = obj.o
     pos, J = obj._kin(x, True)
     n = o.opt_dof
@@ -108,7 +109,8 @@ def _ggn_hessian(obj, x):
     H += _fold(o, o.robot.link_position_hessian_contraction(o.link_ids, gpos))
     if o.type == "position":
         d = pos - obj.target
-        w = np.where(np.abs(d) < beta, 1.0 / beta, 0.0) / d.size
+        a = np.abs(d)
+        w = np.where(a < beta, 1.0 / beta, 1.0 / np.maximum(a, beta) if majoriser else 0.0) / d.size
         H += np.einsum("lc,lci,lcj->ij", w, J, J)
         return H
     Jv = J[o.task_sel] - J[o.origin_sel]  # (m,3,n)
