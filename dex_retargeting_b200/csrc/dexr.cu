@@ -148,17 +148,7 @@ __device__ __forceinline__ void frames_group(const FrameArgs& a, int first_tile)
         in.last = s_last + ci * a.dm.n_var;
         in.fixed = s_fixed + ci * a.dm.n_fixed;
         in.projected = a.io.projected ? a.io.projected + f * a.dm.len_proj : nullptr;
-        sv.lam_carry = a.io.damping_io ? a.io.damping_io[f] : 0.f;  // (every lane of the group reads the frame's word)
-        const int status = sv.solve(in, active);
-        if (active) {
-          if (sv.var >= 0) a.io.qpos_out[f * a.dm.n_var + sv.var] = sv.x;
-          if (a.io.robot_qpos_out && sv.l < a.dm.dof) a.io.robot_qpos_out[f * a.dm.dof + sv.l] = sv.q;
-          if (sv.l == 0) {
-            if (a.io.status_out) a.io.status_out[f] = status;
-            if (a.io.cost_out) a.io.cost_out[f] = sv.F;
-            if (a.io.damping_io) a.io.damping_io[f] = sv.lam_carry;
-          }
-        }
+        solve_frame(sv, in, a.io, a.dm, f, active);
       }
       __syncwarp();
       if (lane == 0) mbar_arrive(&empty[stage]);
@@ -183,7 +173,7 @@ __global__ void __launch_bounds__((NCW + 1) * 32, 1) dexr_frames_kernel(const Fr
 constexpr int kMaxGroups = DEXR_MAX_GROUPS;
 struct MultiArgs {
   int n_groups;
-  int kind[kMaxGroups];  // 0: <16,4>  1: <16,0>  2: <32,-1>  3: <32,0>
+  int kind[kMaxGroups];  // SolverKind
   FrameArgs g[kMaxGroups];
 };
 
@@ -206,9 +196,9 @@ __global__ void __launch_bounds__((NCW + 1) * 32, 1) dexr_frames_multi_kernel(co
     const FrameArgs& a = m.g[gi];
     const int first = (int)((blockIdx.x + gridDim.x - rot) % gridDim.x);
     switch (m.kind[gi]) {
-      case 0: frames_group_call<16, 4, NCW>(a, first); break;
-      case 1: frames_group_call<16, 0, NCW>(a, first); break;
-      case 2: frames_group_call<32, -1, NCW>(a, first); break;
+      case kBlock16: frames_group_call<16, 4, NCW>(a, first); break;
+      case kDense16: frames_group_call<16, 0, NCW>(a, first); break;
+      case kArrow32: frames_group_call<32, -1, NCW>(a, first); break;
       default: frames_group_call<32, 0, NCW>(a, first); break;
     }
     rot = (rot + a.ntiles) % gridDim.x;
@@ -226,87 +216,26 @@ __global__ void __launch_bounds__(NW * 32, 1) dexr_sequences_kernel(const SeqArg
   __syncthreads();
 
   constexpr int GPW = 32 / G;
-  constexpr int KPL = (3 * DEXR_NUM_KEYPOINTS + G - 1) / G;  // keypoint floats per lane
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
   const int lane = threadIdx.x & 31;
   const int gid = warp * GPW + (lane / G);               // scratch slot of this group of lanes
+  const int slots_per_cta = NW * a.spw;
+  const uint32_t scratch_off = (uint32_t)(a.scratch_off + gid * Scratch<G>::kStreamFloats * 4);
+  float* kpbuf = reinterpret_cast<float*>(smem + scratch_off) + Scratch<G>::kFloats;  // 63 floats: current keypoints
   const int slot = a.spw == GPW ? gid : warp;            // which of the CTA's stream slots this group serves
   const bool first = (lane / G) == 0;
   const bool owner = a.spw == GPW || first;              // the group that reads and writes the stream's state
   const bool works = owner || a.duo;                     // (scarce streams, 16 lanes: the second half-warp helps the first)
-  const int slots_per_cta = NW * a.spw;
-  const uint32_t scratch_off = (uint32_t)(a.scratch_off + gid * (Scratch<G>::kFloats + 64) * 4);
-  float* kpbuf = reinterpret_cast<float*>(smem + scratch_off) + Scratch<G>::kFloats;  // 63 floats: current keypoints
   Solver<G, BW> sv;
   sv.init(a.table, a.dm, scratch_off, a.prm, lane);
   if (G == 16 && a.duo) sv.duo = lane / G;
-  const int l = sv.l;
   const bool use_filter = a.prm.lp_alpha >= 0.f && a.prm.lp_alpha <= 1.f;
 
   // Streams are dealt round-robin over CTAs (stream = blockIdx + gridDim * slot): with few streams every SM gets
   // one or two warps instead of a few SMs getting eight -- the path is latency bound per stream.
   for (long long base = 0; base < a.S; base += (long long)gridDim.x * slots_per_cta) {
-    // all groups of a warp must walk the time loop together (warp-wide shuffles inside solve)
     const long long s = base + (long long)slot * gridDim.x + blockIdx.x;
-    const bool active = works && s < a.S;   // solves (and, in duo mode, reads the same state as the owner half)
-    const bool writes = owner && s < a.S;   // stores results and state
-    const long long sc = active ? s : a.S - 1;
-    float last = 0.f, fy = 0.f;
-    int finit = 0;
-    if (active && sv.var >= 0) last = a.io.last_qpos[sc * a.dm.n_var + sv.var];
-    if (active && use_filter && l < a.dm.dof) fy = a.io.filter_state[sc * a.dm.dof + l];
-    if (active && use_filter) finit = a.io.filter_init[sc];
-    sv.lam_carry = (active && a.io.damping_state) ? a.io.damping_state[sc] : 0.f;  // then carried by solve() from frame to frame
-    const float* kp_stream = a.io.keypoints + sc * a.steps * (3 * DEXR_NUM_KEYPOINTS);
-    float pre[KPL];
-#pragma unroll
-    for (int j = 0; j < KPL; ++j) {
-      const int e = l + j * G;
-      pre[j] = (e < 3 * DEXR_NUM_KEYPOINTS) ? kp_stream[e] : 0.f;
-    }
-    for (int t = 0; t < a.steps; ++t) {
-#pragma unroll
-      for (int j = 0; j < KPL; ++j) {
-        const int e = l + j * G;
-        if (e < 3 * DEXR_NUM_KEYPOINTS) kpbuf[e] = pre[j];
-      }
-      if (t + 1 < a.steps) {
-        const float* nxt = kp_stream + (long long)(t + 1) * (3 * DEXR_NUM_KEYPOINTS);
-#pragma unroll
-        for (int j = 0; j < KPL; ++j) {
-          const int e = l + j * G;
-          pre[j] = (e < 3 * DEXR_NUM_KEYPOINTS) ? nxt[e] : 0.f;
-        }
-      }
-      // stash the warm start where solve() reads it: reuse the tail of kpbuf (floats 63 is pad) -> use at()
-      __syncwarp();
-      FrameInputs in;
-      in.kp = kpbuf;
-      in.ref = nullptr;
-      in.fixed = a.dm.n_fixed > 0 ? a.io.fixed_qpos + (sc * a.steps + t) * a.dm.n_fixed : nullptr;
-      in.last = nullptr;  // warm start comes from the register `x` (previous solution)
-      in.projected = a.io.projected ? a.io.projected + sc * a.dm.len_proj : nullptr;
-      sv.x = last;
-      const int status = sv.solve(in, active);
-      last = sv.x;  // unfiltered solution is the next warm start (seq_retarget.py:124)
-      float out = sv.q;
-      if (use_filter) {  // optimizer_utils.py:7-13
-        fy = finit ? fmaf(a.prm.lp_alpha, out - fy, fy) : out;
-        finit = 1;
-        out = fy;
-      }
-      if (writes) {
-        if (l < a.dm.dof) a.io.robot_qpos_out[(sc * a.steps + t) * a.dm.dof + l] = out;
-        if (l == 0 && a.io.status_out) a.io.status_out[sc * a.steps + t] = status;
-      }
-      __syncwarp();
-    }
-    if (writes) {
-      if (sv.var >= 0) a.io.last_qpos[sc * a.dm.n_var + sv.var] = last;
-      if (use_filter && l < a.dm.dof) a.io.filter_state[sc * a.dm.dof + l] = fy;
-      if (use_filter && l == 0) a.io.filter_init[sc] = (uint8_t)finit;
-      if (a.io.damping_state && l == 0) a.io.damping_state[sc] = sv.lam_carry;
-    }
+    solve_stream(sv, a.io, a.dm, a.prm, a.S, a.steps, s, works && s < a.S, owner && s < a.S, kpbuf, use_filter);
   }
 }
 
@@ -443,9 +372,7 @@ struct dexr_robot {
   size_t stage_bytes = 0;
 };
 
-template <int G> struct FramesCfg {
-  static constexpr int kMaxTile = (G == 16) ? 64 : 32;  // frames per ring stage (shared memory budget)
-};
+static int frames_max_tile(int lanes) { return lanes == 16 ? 64 : 32; }  // frames per ring stage (shared memory budget)
 constexpr int kSeqNW = 8;       // warps per CTA (sequences kernel)
 
 static int validate_table(const dexr_table_t* t) {
@@ -643,16 +570,6 @@ static int check_params(const dexr_params_t* p) {
 
 static inline int round_up(int v, int m) { return (v + m - 1) / m * m; }
 
-static Dims make_dims(const dexr_table_t& t) {
-  Dims d;
-  d.dof = t.dof; d.n_var = t.n_var; d.n_fixed = t.n_fixed; d.n_links = t.n_links; d.n_res = t.n_res; d.loss = t.loss;
-  d.n_rounds = t.n_rounds; d.has_mimic = t.has_mimic; d.num_fingers = t.num_fingers; d.len_proj = t.len_proj;
-  d.len_s1 = t.len_s1;
-  d.block_width = t.block_width;
-  d.trunk = t.arrow > 0 ? t.arrow - 1 : 0;
-  return d;
-}
-
 // DEXR_ARROW=0 forces the dense factorisation for tables that qualify for the arrow one.  Read per call (a getenv is
 // nanoseconds against a launch) so that tests can compare the two inside one process.
 static bool arrow_enabled() {
@@ -676,15 +593,16 @@ static int fill_frame_args(const dexr_robot* r, const dexr_params_t* prm, const 
   // the CTA count instead of always using the largest tile (B = 6144 on 132 SMs: 192 tiles of 32 leave 72 CTAs with one
   // tile and 60 with two -- 73 % efficiency; 256 tiles of 24 give all but 8 CTAs two).
   const long long per = (B + slots - 1) / slots;                                            // frames per CTA
-  const long long rounds = std::max<long long>(1, (per + FramesCfg<G>::kMaxTile - 1) / FramesCfg<G>::kMaxTile);
-  int T = (int)std::min<long long>(FramesCfg<G>::kMaxTile, std::max<long long>(4, (per + rounds - 1) / rounds));
+  const int max_tile = frames_max_tile(G);
+  const long long rounds = std::max<long long>(1, (per + max_tile - 1) / max_tile);
+  int T = (int)std::min<long long>(max_tile, std::max<long long>(4, (per + rounds - 1) / rounds));
   T = round_up(T, 4);
   // A CTA solves NCW x (32 / G) frames at a time.  When its whole share fits one such round, rounding the tile up to the
   // bulk-copy granularity must not push it into a second, nearly empty round (Shadow, 2048 frames: 14 per CTA -> 16 on 15
   // warps): keep the exact count, the producer then stages the tile with plain loads.
   constexpr int kRound = NCW * (32 / G);
   if (per <= kRound && T > kRound) T = (int)per;
-  if (tile > 0) T = std::min(tile, FramesCfg<G>::kMaxTile);  // mixed launches size the tiles of all groups together
+  if (tile > 0) T = std::min(tile, max_tile);  // mixed launches size the tiles of all groups together
   a.T = T;
   a.ntiles = (int)((B + T - 1) / T);
   auto aligned16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; };
@@ -748,24 +666,13 @@ static int launch_frames_warps(int warps, dexr_robot* r, const dexr_params_t* pr
   return launch_frames<G, BW, 15>(r, prm, io, B, stream, slots, tile);
 }
 
-static int solver_kind(const dexr_table_t& t);
-
 static int launch_frames_kind(dexr_robot* r, const dexr_params_t* prm, const dexr_frames_t* io, long long B, cudaStream_t stream,
                               int slots = 0, int tile = 0) {
-  const int k = solver_kind(r->host);
+  const SolverKind k = solver_kind(r->host, arrow_enabled());
   const int warps = frames_warps()[k];
-  switch (k) {
-    case 0: return launch_frames_warps<16, 4>(warps, r, prm, io, B, stream, slots, tile);   // decoupled 4-joint fingers: block diagonal
-    case 1: return launch_frames_warps<16, 0>(warps, r, prm, io, B, stream, slots, tile);   // dense, 16 lanes
-    case 2: return launch_frames_warps<32, -1>(warps, r, prm, io, B, stream, slots, tile);  // trunk + decoupled fingers: arrow
-    default: return launch_frames_warps<32, 0>(warps, r, prm, io, B, stream, slots, tile);  // dense, 32 lanes
-  }
-}
-
-// Which solver instantiation a table runs on: 0 <16,4> block diagonal, 1 <16,0> dense, 2 <32,-1> arrow, 3 <32,0> dense.
-static int solver_kind(const dexr_table_t& t) {
-  if (t.dof <= 16) return t.block_width == 4 ? 0 : 1;
-  return (t.arrow > 0 && arrow_enabled()) ? 2 : 3;
+  return with_solver(k, [&](auto s) {
+    return launch_frames_warps<decltype(s)::G, decltype(s)::BW>(warps, r, prm, io, B, stream, slots, tile);
+  });
 }
 
 static int check_frames_io(const dexr_table_t& t, const dexr_frames_t* io, const dexr_params_t* prm) {
@@ -773,6 +680,14 @@ static int check_frames_io(const dexr_table_t& t, const dexr_frames_t* io, const
     return fail(DEXR_E_INVALID, "exactly one of keypoints / ref_value must be given");
   if (prm->preprocess != 0 && !io->keypoints) return fail(DEXR_E_INVALID, "preprocess needs raw keypoints, not ref_value");
   if (!io->last_qpos || !io->qpos_out) return fail(DEXR_E_INVALID, "last_qpos and qpos_out are required");
+  if (t.n_fixed > 0 && !io->fixed_qpos) return fail(DEXR_E_INVALID, "robot has %d fixed joints but fixed_qpos is NULL", t.n_fixed);
+  return 0;
+}
+
+static int check_sequences_io(const dexr_table_t& t, const dexr_sequences_t* io, const dexr_params_t* prm) {
+  if (!io->keypoints || !io->last_qpos || !io->robot_qpos_out) return fail(DEXR_E_INVALID, "keypoints, last_qpos, robot_qpos_out required");
+  const bool use_filter = prm->lp_alpha >= 0.f && prm->lp_alpha <= 1.f;
+  if (use_filter && (!io->filter_state || !io->filter_init)) return fail(DEXR_E_INVALID, "low-pass filter needs filter_state and filter_init");
   if (t.n_fixed > 0 && !io->fixed_qpos) return fail(DEXR_E_INVALID, "robot has %d fixed joints but fixed_qpos is NULL", t.n_fixed);
   return 0;
 }
@@ -795,10 +710,10 @@ extern "C" int dexr_solve_frames_multi(const dexr_group_t* groups, int32_t num_g
     if (int e = check_frames_io(r->host, &g.io, g.params)) return e;
     if (device < 0) { device = r->device; sms = r->num_sms; first = r; }
     if (r->device != device) return fail(DEXR_E_INVALID, "group %d lives on device %d, group 0 on device %d: one launch, one device", i, r->device, device);
-    const int k = solver_kind(r->host);
+    const SolverKind k = solver_kind(r->host, arrow_enabled());
     FrameArgs& a = m.g[m.n_groups];
-    const int need = k <= 1 ? fill_frame_args<16, NCW>(r, g.params, &g.io, g.num_frames, sms, a)
-                            : fill_frame_args<32, NCW>(r, g.params, &g.io, g.num_frames, sms, a);
+    const int need = kind_lanes(k) == 16 ? fill_frame_args<16, NCW>(r, g.params, &g.io, g.num_frames, sms, a)
+                                         : fill_frame_args<32, NCW>(r, g.params, &g.io, g.num_frames, sms, a);
     smem = std::max(smem, need);
     m.kind[m.n_groups++] = k;
     tiles += a.ntiles;
@@ -858,10 +773,10 @@ extern "C" int dexr_solve_frames_multi(const dexr_group_t* groups, int32_t num_g
   Plan plan[DEXR_MAX_GROUPS];
   int n_plan = 0;
   long long R = 0;
-  auto round_of = [](int kind) { return (frames_warps()[kind] - 1) * (kind <= 1 ? 2 : 1); };
+  auto round_of = [](int kind) { return (frames_warps()[kind] - 1) * (32 / kind_lanes(kind)); };
   for (int i = 0; i < num_groups; ++i) {
     if (groups[i].num_frames == 0) continue;
-    const int k = solver_kind(groups[i].robot->host);
+    const int k = solver_kind(groups[i].robot->host, arrow_enabled());
     plan[n_plan++] = Plan{i, k, 0, 0};
     R += (groups[i].num_frames + round_of(k) - 1) / round_of(k);
   }
@@ -874,7 +789,7 @@ extern "C" int dexr_solve_frames_multi(const dexr_group_t* groups, int32_t num_g
     for (int j = 0; j < n_plan; ++j) {
       Plan& p = plan[j];
       const long long B = groups[p.group].num_frames;
-      const int S = round_of(p.kind), max_tile = p.kind <= 1 ? FramesCfg<16>::kMaxTile : FramesCfg<32>::kMaxTile;
+      const int S = round_of(p.kind), max_tile = frames_max_tile(kind_lanes(p.kind));
       long long per = R <= sms ? std::max<long long>(1, (S * R + sms - 1) / sms) : r * S;  // frames per CTA
       if (per <= max_tile) {                                 // one tile per CTA
         p.tile = (int)(per > S ? (per & ~3LL) : per);  // one round: exactly the frames the warps hold (plain loads if not 4 | tile)
@@ -924,8 +839,7 @@ static int launch_sequences(dexr_robot* r, const dexr_params_t* prm, const dexr_
   const dexr_table_t& t = r->host;
   SeqArgs a{};
   a.table = r->table_dev;
-  a.prm = *prm;
-  a.prm.clip_init = 1;  // SeqRetargeting.retarget always clips the warm start (seq_retarget.py:118-120)
+  a.prm = sequence_params(*prm);
   a.io = *io;
   a.S = S;
   a.steps = steps;
@@ -933,7 +847,7 @@ static int launch_sequences(dexr_robot* r, const dexr_params_t* prm, const dexr_
   a.scratch_off = round_up((int)sizeof(SharedTable), 16);
   constexpr int GPW = 32 / G;
   const int groups = kSeqNW * GPW;
-  const int smem = a.scratch_off + groups * (Scratch<G>::kFloats + 64) * 4;
+  const int smem = a.scratch_off + groups * Scratch<G>::kStreamFloats * 4;
   auto kern = dexr_sequences_kernel<G, BW, kSeqNW>;
   CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
   // A stream is serial in time and latency bound, so streams are spread over as many warps and SMs as there are: while one
@@ -963,21 +877,13 @@ extern "C" int dexr_solve_sequences(const dexr_robot_t* robot, const dexr_params
   if (num_streams < 0 || num_steps < 0 || num_steps > INT32_MAX) return fail(DEXR_E_INVALID, "bad sizes");
   if (num_streams == 0 || num_steps == 0) return 0;
   if (int e = check_params(params)) return e;
-  const dexr_table_t& t = robot->host;
-  if (!io->keypoints || !io->last_qpos || !io->robot_qpos_out) return fail(DEXR_E_INVALID, "keypoints, last_qpos, robot_qpos_out required");
-  const bool use_filter = params->lp_alpha >= 0.f && params->lp_alpha <= 1.f;
-  if (use_filter && (!io->filter_state || !io->filter_init)) return fail(DEXR_E_INVALID, "low-pass filter needs filter_state and filter_init");
-  if (t.n_fixed > 0 && !io->fixed_qpos) return fail(DEXR_E_INVALID, "robot has %d fixed joints but fixed_qpos is NULL", t.n_fixed);
+  if (int e = check_sequences_io(robot->host, io, params)) return e;
   DEVICE_SCOPE(robot->device);
   dexr_robot* r = const_cast<dexr_robot*>(robot);
   cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
-  if (t.dof <= 16) {
-    if (t.block_width == 4) return launch_sequences<16, 4>(r, params, io, num_streams, (int)num_steps, stream);
-    return launch_sequences<16, 0>(r, params, io, num_streams, (int)num_steps, stream);
-  }
-  const bool no_arrow = !arrow_enabled();
-  if (t.arrow > 0 && !no_arrow) return launch_sequences<32, -1>(r, params, io, num_streams, (int)num_steps, stream);
-  return launch_sequences<32, 0>(r, params, io, num_streams, (int)num_steps, stream);
+  return with_solver(solver_kind(r->host, arrow_enabled()), [&](auto s) {
+    return launch_sequences<decltype(s)::G, decltype(s)::BW>(r, params, io, num_streams, (int)num_steps, stream);
+  });
 }
 
 extern "C" {
@@ -1011,12 +917,9 @@ int dexr_solve_frames_host(dexr_robot_t* robot, const dexr_params_t* params, con
   if (!robot || !params || !h) return fail(DEXR_E_INVALID, "dexr_solve_frames_host: null argument");
   if (B < 0) return fail(DEXR_E_INVALID, "num_frames < 0");
   if (B == 0) return 0;
-  if ((h->keypoints != nullptr) == (h->ref_value != nullptr))
-    return fail(DEXR_E_INVALID, "exactly one of keypoints / ref_value must be given");
-  if (!h->last_qpos || !h->qpos_out) return fail(DEXR_E_INVALID, "last_qpos and qpos_out are required");
-  std::lock_guard<std::mutex> lock(robot->mu);
   const dexr_table_t& t = robot->host;
-  if (t.n_fixed > 0 && !h->fixed_qpos) return fail(DEXR_E_INVALID, "fixed_qpos is NULL");
+  if (int e = check_frames_io(t, h, params)) return e;
+  std::lock_guard<std::mutex> lock(robot->mu);
   DEVICE_SCOPE(robot->device);
   const int in_row = h->keypoints ? 3 * DEXR_NUM_KEYPOINTS : 3 * t.n_res;
   if (!robot->streams[0]) CUDA_TRY(cudaStreamCreateWithFlags(&robot->streams[0], cudaStreamNonBlocking));

@@ -213,6 +213,16 @@ struct Dims {
   int trunk;        // arrow mode only: number of trunk lanes (lanes 0..trunk-1), see Solver
 };
 
+inline Dims make_dims(const dexr_table_t& t) {
+  Dims d;
+  d.dof = t.dof; d.n_var = t.n_var; d.n_fixed = t.n_fixed; d.n_links = t.n_links; d.n_res = t.n_res; d.loss = t.loss;
+  d.n_rounds = t.n_rounds; d.has_mimic = t.has_mimic; d.num_fingers = t.num_fingers; d.len_proj = t.len_proj;
+  d.len_s1 = t.len_s1;
+  d.block_width = t.block_width;
+  d.trunk = t.arrow > 0 ? t.arrow - 1 : 0;
+  return d;
+}
+
 // ------------------------------------------------------------------------------------------------
 // uniform (per CTA) slice of the robot table kept in shared memory
 // ------------------------------------------------------------------------------------------------
@@ -332,6 +342,7 @@ struct Scratch {
   static constexpr int kHb = kU + kUSize;                       // [NP][NP]   Hessian backup, column per lane
   static constexpr int kLcol = kHb + NP * NP;                   // [NP][NP+1] L^T rows, conflict-free column reads (also mimic-fold temp)
   static constexpr int kFloats = ((kLcol + NP * (NP + 1) + 3) / 4) * 4;
+  static constexpr int kStreamFloats = kFloats + 64;  // sequences: followed by the current frame's 63 keypoint floats
 };
 
 // ------------------------------------------------------------------------------------------------
@@ -1300,5 +1311,137 @@ struct Solver {
     return status;
   }
 };
+
+// ------------------------------------------------------------------------------------------------
+// which Solver instantiation runs a table
+// ------------------------------------------------------------------------------------------------
+// The values index per-kind settings (DEXR_FRAMES_WARPS) and order the kinds from fastest to slowest.
+enum SolverKind {
+  kBlock16 = 0,  // <16, 4>: decoupled 4-joint fingers, block-diagonal Hessian
+  kDense16 = 1,  // <16, 0>
+  kArrow32 = 2,  // <32, -1>: trunk + decoupled fingers, arrow Hessian
+  kDense32 = 3,  // <32, 0>
+};
+
+// use_arrow = false runs arrow-qualified tables on the dense 32-lane solver.
+inline SolverKind solver_kind(const dexr_table_t& t, bool use_arrow) {
+  if (t.dof <= 16) return t.block_width == 4 ? kBlock16 : kDense16;
+  return (t.arrow > 0 && use_arrow) ? kArrow32 : kDense32;
+}
+
+inline int kind_lanes(int kind) { return kind <= kDense16 ? 16 : 32; }
+
+template <int G_, int BW_>
+struct SolverTag {
+  static constexpr int G = G_, BW = BW_;
+};
+
+// f(SolverTag<G, BW>{}) for the instantiation of `kind`.
+template <class F>
+auto with_solver(SolverKind kind, F&& f) {
+  switch (kind) {
+    case kBlock16: return f(SolverTag<16, 4>{});
+    case kDense16: return f(SolverTag<16, 0>{});
+    case kArrow32: return f(SolverTag<32, -1>{});
+    default: return f(SolverTag<32, 0>{});
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
+// frame and stream drivers of the kernels (dexr.cu), also run by the host emulation (tests/emu)
+// ------------------------------------------------------------------------------------------------
+// One frame of a batch: solve from the frame's carried damping, then write its outputs.  `dm` is the kernel argument's, not
+// sv.dm: read from the constant bank, it keeps the register allocation of the frames kernels.
+template <int G, int BW>
+__device__ __forceinline__ void solve_frame(Solver<G, BW>& sv, const FrameInputs& in, const dexr_frames_t& io, const Dims& dm,
+                                            long long f, bool active) {
+  sv.lam_carry = io.damping_io ? io.damping_io[f] : 0.f;  // (every lane of the group reads the frame's word)
+  const int status = sv.solve(in, active);
+  if (active) {
+    if (sv.var >= 0) io.qpos_out[f * dm.n_var + sv.var] = sv.x;
+    if (io.robot_qpos_out && sv.l < dm.dof) io.robot_qpos_out[f * dm.dof + sv.l] = sv.q;
+    if (sv.l == 0) {
+      if (io.status_out) io.status_out[f] = status;
+      if (io.cost_out) io.cost_out[f] = sv.F;
+      if (io.damping_io) io.damping_io[f] = sv.lam_carry;
+    }
+  }
+}
+
+// SeqRetargeting.retarget always clips the warm start (seq_retarget.py:118-120).
+inline dexr_params_t sequence_params(dexr_params_t p) {
+  p.clip_init = 1;
+  return p;
+}
+
+// One stream s of S: its `steps` frames in order (seq_retarget.py:112-134), warm start and filter carried in registers.  The
+// frame's keypoints are staged in `kpbuf` (63 floats of shared memory), the next frame's are prefetched into registers
+// meanwhile.  Every group of a warp walks the time loop (warp-wide shuffles inside solve); a group that is not `active` runs
+// it on stream S - 1, and only a group that `writes` stores results and state.  `use_filter`: prm.lp_alpha in [0, 1].
+// dm, prm, S and steps are the kernel argument's and `use_filter` is computed once per thread: taken by value here, or
+// recomputed per stream, they change the register allocation of the sequences kernels.
+template <int G, int BW>
+__device__ __forceinline__ void solve_stream(Solver<G, BW>& sv, const dexr_sequences_t& io, const Dims& dm,
+                                             const dexr_params_t& prm, const long long& S, const int& steps, long long s,
+                                             bool active, bool writes, float* kpbuf, bool use_filter) {
+  constexpr int KPL = (3 * DEXR_NUM_KEYPOINTS + G - 1) / G;  // keypoint floats per lane
+  const int l = sv.l;
+  const long long sc = active ? s : S - 1;
+  float last = 0.f, fy = 0.f;
+  int finit = 0;
+  if (active && sv.var >= 0) last = io.last_qpos[sc * dm.n_var + sv.var];
+  if (active && use_filter && l < dm.dof) fy = io.filter_state[sc * dm.dof + l];
+  if (active && use_filter) finit = io.filter_init[sc];
+  sv.lam_carry = (active && io.damping_state) ? io.damping_state[sc] : 0.f;  // then carried by solve() from frame to frame
+  const float* kp_stream = io.keypoints + sc * steps * (3 * DEXR_NUM_KEYPOINTS);
+  float pre[KPL];
+#pragma unroll
+  for (int j = 0; j < KPL; ++j) {
+    const int e = l + j * G;
+    pre[j] = (e < 3 * DEXR_NUM_KEYPOINTS) ? kp_stream[e] : 0.f;
+  }
+  for (int t = 0; t < steps; ++t) {
+#pragma unroll
+    for (int j = 0; j < KPL; ++j) {
+      const int e = l + j * G;
+      if (e < 3 * DEXR_NUM_KEYPOINTS) kpbuf[e] = pre[j];
+    }
+    if (t + 1 < steps) {
+      const float* nxt = kp_stream + (long long)(t + 1) * (3 * DEXR_NUM_KEYPOINTS);
+#pragma unroll
+      for (int j = 0; j < KPL; ++j) {
+        const int e = l + j * G;
+        pre[j] = (e < 3 * DEXR_NUM_KEYPOINTS) ? nxt[e] : 0.f;
+      }
+    }
+    __syncwarp();
+    FrameInputs in;
+    in.kp = kpbuf;
+    in.ref = nullptr;
+    in.fixed = dm.n_fixed > 0 ? io.fixed_qpos + (sc * steps + t) * dm.n_fixed : nullptr;
+    in.last = nullptr;  // warm start comes from the register `x` (previous solution)
+    in.projected = io.projected ? io.projected + sc * dm.len_proj : nullptr;
+    sv.x = last;
+    const int status = sv.solve(in, active);
+    last = sv.x;  // unfiltered solution is the next warm start (seq_retarget.py:124)
+    float out = sv.q;
+    if (use_filter) {  // optimizer_utils.py:7-13
+      fy = finit ? fmaf(prm.lp_alpha, out - fy, fy) : out;
+      finit = 1;
+      out = fy;
+    }
+    if (writes) {
+      if (l < dm.dof) io.robot_qpos_out[(sc * steps + t) * dm.dof + l] = out;
+      if (l == 0 && io.status_out) io.status_out[sc * steps + t] = status;
+    }
+    __syncwarp();
+  }
+  if (writes) {
+    if (sv.var >= 0) io.last_qpos[sc * dm.n_var + sv.var] = last;
+    if (use_filter && l < dm.dof) io.filter_state[sc * dm.dof + l] = fy;
+    if (use_filter && l == 0) io.filter_init[sc] = (uint8_t)finit;
+    if (io.damping_state && l == 0) io.damping_state[sc] = sv.lam_carry;
+  }
+}
 
 }  // namespace dexr

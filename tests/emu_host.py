@@ -17,7 +17,7 @@ SOURCES = [EMU / "emu_driver.cpp", EMU / "warp_shim.h", ROOT / "dex_retargeting_
 
 @lru_cache(maxsize=None)
 def load(defines: tuple = ()):
-    """defines: compile-time experiment switches, e.g. ("DEXR_EXP_MERGEDRES",)."""
+    """defines: compile-time experiment switches, e.g. ("DEXR_EXP_FASTSINCOS",)."""
     OUT.mkdir(exist_ok=True)
     tag = "_".join(d.replace("DEXR_EXP_", "").lower() for d in defines) or "default"
     so = OUT / f"libdexr_emu_{tag}.so"
@@ -56,11 +56,15 @@ def solve_frames(opt, last_qpos, keypoints=None, ref_value=None, fixed_qpos=None
     err = C.create_string_buffer(600)
 
     def ptr(a):
-        return None if a is None else a.ctypes.data_as(C.c_void_p)
+        return None if a is None else a.ctypes.data
 
     full = np.zeros((B, table.dof), np.float32) if want_robot_qpos else None
-    rc = lib.emu_solve_frames(C.byref(table), C.byref(prm), C.c_int(int(use_arrow)), ptr(kp), ptr(ref), ptr(last), ptr(fixed),
-                              ptr(projected), C.c_longlong(B), ptr(out), ptr(full), ptr(status), ptr(cost), ptr(damping), err, C.c_int(600))
+    io = N.DexrFrames()
+    io.keypoints, io.ref_value, io.last_qpos, io.fixed_qpos = ptr(kp), ptr(ref), ptr(last), ptr(fixed)
+    io.projected, io.qpos_out, io.robot_qpos_out = ptr(projected), ptr(out), ptr(full)
+    io.status_out, io.cost_out, io.damping_io = ptr(status), ptr(cost), ptr(damping)
+    rc = lib.emu_solve_frames(C.byref(table), C.byref(prm), C.c_int(int(use_arrow)), C.byref(io), C.c_longlong(B), err,
+                              C.c_int(600))
     if rc != 0:
         raise RuntimeError(f"host emulation failed ({rc}): {err.value.decode()}")
     return (out, status, cost, full) if want_robot_qpos else (out, status, cost)

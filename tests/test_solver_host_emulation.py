@@ -76,8 +76,8 @@ def test_solver_source_matches_oracle(key, use_arrow, n):
 @pytest.mark.parametrize("defines", VARIANTS, ids=lambda d: "+".join(x.replace("DEXR_EXP_", "").lower() for x in d))
 @pytest.mark.parametrize("key,use_arrow,n", CASES)
 def test_experiment_switches(key, use_arrow, n, defines):
-    """Every compile-time experiment (csrc/dexr_kernels.cuh "Experiment switches") solves the same problems: the noise
-    floor and the PD fallback take another iteration path and must land on the oracle's minimiser."""
+    """Every compile-time experiment (csrc/dexr_kernels.cuh "Experiment switches") solves the same problems:
+    DEXR_EXP_FASTSINCOS takes another iteration path and must land on the oracle's minimiser."""
     _, _, _, _, q0, s0, c0, p0 = emulate(key, n, use_arrow)
     o, refs, fixed, x0, q, status, cost, proj = emulate(key, n, use_arrow, defines)
     assert np.all((status >> 24) == 0)
@@ -121,7 +121,7 @@ def test_non_finite_input_is_flagged_and_isolated():
                                            ("teleop/schunk_svh_hand_right", True)])
 def test_streams_recurrence(key, vs_oracle):
     """The stream recurrence around the same solve() (warm start carried in the lane's register, clip, unfiltered solution =
-    next warm start, low-pass filter, DexPilot flags in place; restated from dexr_sequences_kernel in tests/emu) equals the
+    next warm start, low-pass filter, DexPilot flags in place: solve_stream, which dexr_sequences_kernel runs) equals the
     frame-by-frame twin through the frames entry bit for bit, and the oracle's SeqRetargeting where basins are unambiguous."""
     from oracle.solvers import OracleSeqRetargeting
 

@@ -6,7 +6,7 @@ Inside the test modules `torch` is a proxy that maps every device to the CPU.  N
 anything that is specific to the kernels of dexr.cu (tile ring, alignment paths), GPU arithmetic in the last bits.
 
   python tests/tools/emu_gpu_tests.py                                   # default build of the solver
-  python tests/tools/emu_gpu_tests.py DEXR_EXP_PDFALLBACK DEXR_EXP_FKNOISE [-k substring]
+  python tests/tools/emu_gpu_tests.py DEXR_EXP_FASTSINCOS [-k substring]
 """
 import itertools
 import os
