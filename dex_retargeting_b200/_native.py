@@ -66,6 +66,16 @@ class DexrSequences(C.Structure):
     ]
 
 
+class DexrEval(C.Structure):
+    """Mirror of `dexr_eval_t`: buffers of one objective evaluation (`dexr_eval_objective`)."""
+
+    _fields_ = [
+        ("keypoints", C.c_void_p), ("ref_value", C.c_void_p), ("fixed_qpos", C.c_void_p), ("qpos", C.c_void_p),
+        ("last_qpos", C.c_void_p), ("projected", C.c_void_p), ("loss_out", C.c_void_p), ("cost_out", C.c_void_p),
+        ("grad_out", C.c_void_p),
+    ]
+
+
 class DexrGroup(C.Structure):
     """Mirror of `dexr_group_t`: one (robot, batch) group of a mixed-robot launch."""
 
@@ -85,7 +95,7 @@ EXPORTS = [
     "dexr_sequences_sizeof", "dexr_default_params",
     "dexr_robot_create", "dexr_robot_create_from_device", "dexr_robot_device_table", "dexr_robot_destroy",
     "dexr_solve_frames", "dexr_solve_frames_multi", "dexr_solve_sequences", "dexr_solve_frames_host", "dexr_get_launch_info",
-    "dexr_preprocess_keypoints",
+    "dexr_preprocess_keypoints", "dexr_eval_sizeof", "dexr_eval_objective",
 ]
 
 _LIB = None
@@ -143,6 +153,13 @@ def load():
             raise DexrError("dexr_frames_t / dexr_sequences_t layout mismatch between library and binding (stale DEXR_LIBRARY?)")
     elif not os.environ.get("DEXR_LIBRARY"):
         raise DexrError(f"{path} does not export dexr_frames_sizeof: rebuild it (python -m dex_retargeting_b200.build --force)")
+    if hasattr(lib, "dexr_eval_sizeof"):
+        lib.dexr_eval_sizeof.restype = C.c_size_t
+        if lib.dexr_eval_sizeof() != C.sizeof(DexrEval):
+            raise DexrError("dexr_eval_t layout mismatch between library and binding (stale DEXR_LIBRARY?)")
+        lib.dexr_eval_objective.argtypes = [C.c_void_p, C.POINTER(DexrParams), C.POINTER(DexrEval), C.c_int64, C.c_void_p]
+    elif not os.environ.get("DEXR_LIBRARY"):
+        raise DexrError(f"{path} does not export dexr_eval_sizeof: rebuild it (python -m dex_retargeting_b200.build --force)")
     # (an older A/B library named by DEXR_LIBRARY reads a prefix of the buffer structs -- fields are only ever appended -- so
     # the single-robot entry points still work with it; dexr_solve_frames_multi, whose groups embed the struct, does not)
     _LIB = lib

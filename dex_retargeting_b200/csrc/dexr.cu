@@ -240,6 +240,49 @@ __global__ void __launch_bounds__(NW * 32, 1) dexr_sequences_kernel(const SeqArg
 }
 
 // ------------------------------------------------------------------------------------------------
+// objective evaluation: one frame per group of G lanes, groups striding over the batch
+// ------------------------------------------------------------------------------------------------
+// One pass over ~0.5 KB per frame with no iteration: inputs are read with plain loads where they lie (no TMA ring), and the
+// table is loaded into shared memory once per CTA.
+constexpr int kEvalWarps = 8;
+
+struct EvalArgs {
+  const dexr_table_t* table;
+  dexr_params_t prm;
+  dexr_eval_t io;
+  long long B;
+  int in_row;  // floats per frame of the kp/ref input (63 or 3m)
+  Dims dm;
+  int scratch_off;
+};
+
+// (a minimum of 2 CTAs per SM: with none, ptxas gives the 32-lane kernel 64 registers and 8 bytes of spills; now 69-71 and none)
+template <int G>
+__global__ void __launch_bounds__(kEvalWarps * 32, 2) dexr_eval_kernel(const EvalArgs a) {
+  load_shared_table(*reinterpret_cast<SharedTable*>(dsmem), a.table);  // (the residual-pass schedule is not read)
+  __syncthreads();
+  constexpr int GPW = 32 / G;
+  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
+  const int lane = threadIdx.x & 31;
+  Solver<G, 0> sv;
+  sv.init(a.table, a.dm, (uint32_t)(a.scratch_off + (warp * GPW + lane / G) * eval_scratch_floats<G>() * 4), a.prm, lane);
+  const bool by_kp = a.io.keypoints != nullptr;
+  const long long step = (long long)gridDim.x * kEvalWarps * GPW;
+  for (long long base = ((long long)blockIdx.x * kEvalWarps + warp) * GPW; base < a.B; base += step) {
+    const long long idx = base + lane / G;
+    const bool active = idx < a.B;
+    const long long f = active ? idx : base;
+    FrameInputs in;
+    in.kp = by_kp ? a.io.keypoints + f * a.in_row : nullptr;
+    in.ref = by_kp ? nullptr : a.io.ref_value + f * a.in_row;
+    in.fixed = a.dm.n_fixed > 0 ? a.io.fixed_qpos + f * a.dm.n_fixed : nullptr;
+    in.last = nullptr;
+    in.projected = a.io.projected ? a.io.projected + f * a.dm.len_proj : nullptr;
+    evaluate_frame(sv, in, a.io, a.dm, f, active);
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
 // keypoint pre-processing (single_hand_detector.py:100-103, 130-158): one thread per frame for the 3x3 frame,
 // tile staged through shared memory so that global loads / stores are coalesced 16-byte accesses
 // ------------------------------------------------------------------------------------------------
@@ -486,6 +529,7 @@ size_t dexr_table_sizeof(void) { return sizeof(dexr_table_t); }
 size_t dexr_params_sizeof(void) { return sizeof(dexr_params_t); }
 size_t dexr_frames_sizeof(void) { return sizeof(dexr_frames_t); }
 size_t dexr_sequences_sizeof(void) { return sizeof(dexr_sequences_t); }
+size_t dexr_eval_sizeof(void) { return sizeof(dexr_eval_t); }
 
 void dexr_default_params(dexr_params_t* p) {
   p->huber_delta = 0.02f;
@@ -690,6 +734,73 @@ static int check_sequences_io(const dexr_table_t& t, const dexr_sequences_t* io,
   if (use_filter && (!io->filter_state || !io->filter_init)) return fail(DEXR_E_INVALID, "low-pass filter needs filter_state and filter_init");
   if (t.n_fixed > 0 && !io->fixed_qpos) return fail(DEXR_E_INVALID, "robot has %d fixed joints but fixed_qpos is NULL", t.n_fixed);
   return 0;
+}
+
+static int check_eval_io(const dexr_table_t& t, const dexr_eval_t* io, const dexr_params_t* prm) {
+  if (const char* msg = eval_io_error(t, *io, *prm)) return fail(DEXR_E_INVALID, "%s", msg);
+  return 0;
+}
+
+// The loss fields of check_params: an evaluation ignores the solver's.
+static int check_loss_params(const dexr_params_t* p) {
+  if (!(p->huber_delta > 0.f)) return fail(DEXR_E_INVALID, "huber_delta must be > 0");
+  if (!(p->norm_delta >= 0.f)) return fail(DEXR_E_INVALID, "norm_delta must be >= 0");
+  if (p->preprocess < 0 || p->preprocess > 2) return fail(DEXR_E_INVALID, "preprocess must be 0 (none), 1 (right hand) or 2 (left hand)");
+  return 0;
+}
+
+// CTAs per SM of the evaluation kernel: as many as are resident at once (registers and shared memory allow), one wave that
+// grid-strides over the batch.  DEXR_EVAL_CTAS_PER_SM (read per call) caps it for A/B runs.  The choice is measured in
+// DESIGN.md section 3 ("Objective evaluation").
+template <int G>
+static int eval_ctas_per_sm(int smem, int* out) {
+  int resident = 0;
+  CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&resident, dexr_eval_kernel<G>, kEvalWarps * 32, smem));
+  int n = std::max(1, resident);
+  if (const char* e = getenv("DEXR_EVAL_CTAS_PER_SM"))
+    if (atoi(e) > 0) n = std::min(n, atoi(e));
+  *out = n;
+  return 0;
+}
+
+template <int G>
+static int launch_eval(dexr_robot* r, const dexr_params_t* prm, const dexr_eval_t* io, long long B, cudaStream_t stream) {
+  const dexr_table_t& t = r->host;
+  EvalArgs a{};
+  a.table = r->table_dev;
+  a.prm = *prm;
+  a.io = *io;
+  a.B = B;
+  a.in_row = io->keypoints ? 3 * DEXR_NUM_KEYPOINTS : 3 * t.n_res;
+  a.dm = make_dims(t);
+  a.scratch_off = round_up((int)sizeof(SharedTable), 16);
+  constexpr int GPW = 32 / G;
+  const int smem = a.scratch_off + kEvalWarps * GPW * eval_scratch_floats<G>() * 4;  // below the 48 KB default
+  int per_sm = 1;
+  if (int e = eval_ctas_per_sm<G>(smem, &per_sm)) return e;
+  const long long ctas = (B + kEvalWarps * GPW - 1) / (kEvalWarps * GPW);
+  const int grid = (int)std::min<long long>(ctas, (long long)r->num_sms * per_sm);
+  dexr_eval_kernel<G><<<grid, kEvalWarps * 32, smem, stream>>>(a);
+  CUDA_TRY(cudaGetLastError());
+  {
+    std::lock_guard<std::mutex> lk(r->info_mu);
+    r->last = dexr_launch_info_t{grid, kEvalWarps * 32, smem, 0, G, kEvalWarps, r->last.kernels_launched + 1};
+  }
+  return 0;
+}
+
+extern "C" int dexr_eval_objective(const dexr_robot_t* robot, const dexr_params_t* params, const dexr_eval_t* io,
+                                   int64_t num_frames, void* cuda_stream) {
+  if (!robot || !params || !io) return fail(DEXR_E_INVALID, "dexr_eval_objective: null argument");
+  if (num_frames < 0) return fail(DEXR_E_INVALID, "num_frames < 0");
+  if (int e = check_eval_io(robot->host, io, params)) return e;
+  if (int e = check_loss_params(params)) return e;
+  if (num_frames == 0) return 0;
+  DEVICE_SCOPE(robot->device);
+  dexr_robot* r = const_cast<dexr_robot*>(robot);
+  cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
+  return eval_lanes(r->host) == 16 ? launch_eval<16>(r, params, io, num_frames, stream)
+                                   : launch_eval<32>(r, params, io, num_frames, stream);
 }
 
 extern "C" int dexr_solve_frames_multi(const dexr_group_t* groups, int32_t num_groups, void* cuda_stream) {

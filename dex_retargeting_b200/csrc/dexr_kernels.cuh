@@ -1444,4 +1444,130 @@ __device__ __forceinline__ void solve_stream(Solver<G, BW>& sv, const dexr_seque
   }
 }
 
+// ------------------------------------------------------------------------------------------------
+// objective evaluation (dexr_eval_objective): value and gradient at a given point, no solve
+// ------------------------------------------------------------------------------------------------
+// The evaluation runs on the dense Solver of the table's lane count.  Block and arrow tables have neither mimic nor fixed
+// joints, so the dense compose_q is exact for them, and with no Hessian to build their instantiations have nothing to add.
+inline int eval_lanes(const dexr_table_t& t) { return t.dof <= 16 ? 16 : 32; }
+
+// An evaluating group only uses the targets and the link positions of its scratch (Scratch<G>::kFr, kLp).
+template <int G>
+__host__ __device__ constexpr int eval_scratch_floats() { return Scratch<G>::kU; }
+
+// The argument checks of dexr_eval_objective that read the robot's table: nullptr, or what is wrong.  Host code, so that the
+// host emulation rejects the same arguments with the same messages.
+inline const char* eval_io_error(const dexr_table_t& t, const dexr_eval_t& io, const dexr_params_t& prm) {
+  if (!io.qpos) return "qpos is required";
+  if ((io.keypoints != nullptr) == (io.ref_value != nullptr)) return "exactly one of keypoints / ref_value must be given";
+  if (prm.preprocess != 0 && !io.keypoints) return "preprocess needs raw keypoints, not ref_value";
+  if (t.n_fixed > 0 && !io.fixed_qpos) return "the robot has fixed joints but fixed_qpos is NULL";
+  return nullptr;
+}
+
+// One frame: the objective at x = qpos[f] as given (no clipping), anchored at last_qpos[f] (or x: no regulariser).  The targets
+// and DexPilot flags are prepared by the same prepare_targets a solve runs.  Writes L(x), L(x) + norm_delta |x - x0|^2 (a
+// fresh sum: solve() carries its F from step to step, so the two differ by a few ulp per accepted iteration) and the gradient
+// of the latter.  `dm` is the kernel argument's (constant bank), as in solve_frame.
+template <int G>
+__device__ __forceinline__ void evaluate_frame(Solver<G, 0>& sv, const FrameInputs& in, const dexr_eval_t& io, const Dims& dm,
+                                               long long f, bool active) {
+  const SharedTable& st = Solver<G, 0>::ST();
+  const int l = sv.l;
+  const bool isvar = sv.var >= 0;
+  float x = 0.f, x0 = 0.f;
+  if (active && isvar) {
+    x = io.qpos[f * dm.n_var + sv.var];
+    x0 = io.last_qpos ? io.last_qpos[f * dm.n_var + sv.var] : x;
+  }
+  const int fixedi = st.fixed_index[l];
+  sv.qfix = (active && fixedi >= 0) ? in.fixed[fixedi] : 0.f;
+  sv.x = x;
+  sv.prepare_targets(in, active);
+  __syncwarp();
+  sv.q = sv.compose_q(x);
+  {
+    float R[9];
+    sv.fk(sv.q, R, sv.p);
+    sv.write_world_links();
+    sv.write_links(R, sv.p, 0);
+    sv.set_world_axis(R);
+  }
+  __syncwarp();
+  sv.x0 = x;  // the regulariser term of every lane is exactly 0 (NaN for a non-finite x): L(x)
+  sv.cost(0, x);
+  const float loss = gsum<G>(sv.cost_lane);
+  sv.x0 = x0;
+  sv.cost(0, x);
+  const float cost = gsum<G>(sv.cost_lane);
+
+  float g = 0.f;
+  if (io.grad_out) {
+    // dL/dq of this lane's joint: over the residuals, the loss derivative (the formulas of solve(): per-coordinate Huber slope,
+    // h'(d) r / d with 0 at d = 0 as torch's norm backward) dotted with this lane's Jacobian column of task minus origin link.
+    // One residual per pass on every lane: solve()'s merged passes and its Hessian are of no use here.
+    const float beta = sv.prm.huber_delta, inv_beta = sv.inv_beta;
+    const bool rev = sv.jtype == 0;
+    const float4* lpc = sv.lp(0);
+    for (int k = 0; k < dm.n_res; ++k) {
+      const int ti = st.res_task[k], oi = st.res_origin[k];
+      const float4 T = sv.fr()[k];
+      const float4 pt = lpc[ti];
+      float rx = pt.x - T.x, ry = pt.y - T.y, rz = pt.z - T.z;
+      float j0 = 0.f, j1 = 0.f, j2 = 0.f;
+      if ((st.link_anc[ti] >> l) & 1u) {
+        if (rev) {
+          const float dx = pt.x - sv.p[0], dy = pt.y - sv.p[1], dz = pt.z - sv.p[2];
+          j0 = sv.a[1] * dz - sv.a[2] * dy; j1 = sv.a[2] * dx - sv.a[0] * dz; j2 = sv.a[0] * dy - sv.a[1] * dx;
+        } else { j0 = sv.a[0]; j1 = sv.a[1]; j2 = sv.a[2]; }
+      }
+      if (oi >= 0) {
+        const float4 po = lpc[oi];
+        rx -= po.x; ry -= po.y; rz -= po.z;
+        if ((st.link_anc[oi] >> l) & 1u) {
+          if (rev) {
+            const float dx = po.x - sv.p[0], dy = po.y - sv.p[1], dz = po.z - sv.p[2];
+            j0 -= sv.a[1] * dz - sv.a[2] * dy; j1 -= sv.a[2] * dx - sv.a[0] * dz; j2 -= sv.a[0] * dy - sv.a[1] * dx;
+          } else { j0 -= sv.a[0]; j1 -= sv.a[1]; j2 -= sv.a[2]; }
+        }
+      }
+      float gx, gy, gz;
+      if (dm.loss == DEXR_LOSS_POSITION) {
+        const float ax_ = fabsf(rx), ay_ = fabsf(ry), az_ = fabsf(rz);
+        const float wx = ax_ < beta ? inv_beta : fast_rcp(ax_);
+        const float wy = ay_ < beta ? inv_beta : fast_rcp(ay_);
+        const float wz = az_ < beta ? inv_beta : fast_rcp(az_);
+        gx = T.w * rx * wx; gy = T.w * ry * wy; gz = T.w * rz * wz;
+      } else {
+        const float d = sqrtf(fmaf(rx, rx, fmaf(ry, ry, rz * rz)));
+        const float invd = d > 1e-30f ? fast_rcp(d) : 0.f;
+        const float hp = d < beta ? d * inv_beta : 1.0f;
+        gx = T.w * hp * (rx * invd); gy = T.w * hp * (ry * invd); gz = T.w * hp * (rz * invd);
+      }
+      g = fmaf(j0, gx, fmaf(j1, gy, fmaf(j2, gz, g)));
+    }
+    // mimic fold g_x = M^T g_q (kinematics_adaptor.py backward_jacobian), as in solve()
+    if (dm.has_mimic) {
+      const int gcount = st.group_count[l];
+      float gx_ = 0.f;
+#pragma unroll
+      for (int k = 0; k < DEXR_MAX_GROUP; ++k) {
+        const bool v = isvar && k < gcount;
+        const float gv = gshfl<G>(g, v ? st.group_lane[l][k] : l);
+        if (v) gx_ = fmaf(st.group_mult[l][k], gv, gx_);
+      }
+      g = gx_;
+    }
+    g = isvar ? fmaf(2.0f * sv.prm.norm_delta, x - x0, g) : 0.f;
+  }
+  if (active) {
+    if (isvar && io.grad_out) io.grad_out[f * dm.n_var + sv.var] = g;
+    if (l == 0) {
+      if (io.loss_out) io.loss_out[f] = loss;
+      if (io.cost_out) io.cost_out[f] = cost;
+    }
+  }
+  __syncwarp();  // the group's next frame rewrites the targets and link positions this one read
+}
+
 }  // namespace dexr

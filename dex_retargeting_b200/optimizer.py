@@ -5,9 +5,13 @@ class names, constructor arguments, attributes (`idx_pin2target`, `idx_pin2fixed
 `target_link_human_indices`, `computed_link_indices`, `origin_link_indices`, ...), the same
 `retarget(ref_value, fixed_qpos, last_qpos) -> float32 (n,)` entry, the same ValueErrors.
 
-What changed underneath: there is no nlopt object and no Python objective closure.  `retarget()` ships
-one frame through the C ABI (`dexr_solve_frames_host`); the new `retarget_batch()` takes torch CUDA
-tensors `[B, ...]` and solves every frame of the batch in ONE kernel launch (`dexr_solve_frames`).
+What changed underneath: there is no nlopt object, and the solve does not go through a Python objective
+closure.  `retarget()` ships one frame through the C ABI (`dexr_solve_frames_host`); the new
+`retarget_batch()` takes torch CUDA tensors `[B, ...]` and solves every frame of the batch in ONE kernel
+launch (`dexr_solve_frames`).  `get_objective_function()` still returns the reference's closure
+`objective(x, grad)`, evaluated on the GPU (`dexr_eval_objective`, one frame per call), and
+`objective_batch()` evaluates value and gradient for a whole batch of given joint vectors in one launch
+(see also `objective.retargeting_cost`, the same as a differentiable torch function).
 The solver minimises the objective whose gradient the reference hands to SLSQP, i.e.
     L(x) + norm_delta * |x - last_qpos|^2      inside [lower - 1e-3, upper + 1e-3]
 to convergence (the reference stops SLSQP early at ftol_abs 1e-5 / 1e-6, optimizer.py:136,239,397).
@@ -359,27 +363,9 @@ class Optimizer:
             raise ValueError("last_qpos is required")
         B = last_qpos.shape[0]
         dev = torch.device("cuda", eng.device)
-
-        def chk(t, shape, dtype, name):
-            if t.device != dev or t.dtype != dtype or not t.is_contiguous() or tuple(t.shape) != tuple(shape):
-                raise ValueError(f"{name}: expected contiguous {dtype} tensor of shape {tuple(shape)} on {dev}, "
-                                 f"got {t.dtype} {tuple(t.shape)} on {t.device}")
-            return t.data_ptr()
-
+        chk = _tensor_check(dev)
         io = N.DexrFrames()
-        m = self.num_residuals
-        if (ref_value is None) == (keypoints is None):
-            raise ValueError("give exactly one of ref_value / keypoints")
-        if keypoints is not None:
-            io.keypoints = chk(keypoints, (B, N.NUM_KEYPOINTS, 3), torch.float32, "keypoints")
-        else:
-            io.ref_value = chk(ref_value, (B, m, 3), torch.float32, "ref_value")
-        io.last_qpos = chk(last_qpos, (B, self.opt_dof), torch.float32, "last_qpos")
-        nf = len(self.idx_pin2fixed)
-        if nf:
-            if fixed_qpos is None:
-                raise ValueError(f"Optimizer has {nf} joints but no fixed_qpos is given")
-            io.fixed_qpos = chk(fixed_qpos, (B, nf), torch.float32, "fixed_qpos")
+        self._batch_targets(io, chk, B, ref_value, keypoints, fixed_qpos, last_qpos=last_qpos)
         if out is None:
             out = torch.empty((B, self.opt_dof), dtype=torch.float32, device=dev)
         io.qpos_out = chk(out, (B, self.opt_dof), torch.float32, "out")
@@ -396,6 +382,127 @@ class Optimizer:
         if raw_hand is not None and keypoints is None:
             raise ValueError("raw_hand needs `keypoints` (raw landmarks), not ref_value")
         return eng, io, self.params(clip_init=clip_init, raw_hand=raw_hand), out, B
+
+    def _batch_targets(self, io, chk, B, ref_value, keypoints, fixed_qpos, last_qpos=None):
+        """The per-frame inputs `dexr_frames_t` and `dexr_eval_t` share: ref_value or keypoints, last_qpos (when given, in
+        that order), fixed_qpos."""
+        import torch
+
+        if (ref_value is None) == (keypoints is None):
+            raise ValueError("give exactly one of ref_value / keypoints")
+        if keypoints is not None:
+            io.keypoints = chk(keypoints, (B, N.NUM_KEYPOINTS, 3), torch.float32, "keypoints")
+        else:
+            io.ref_value = chk(ref_value, (B, self.num_residuals, 3), torch.float32, "ref_value")
+        if last_qpos is not None:
+            io.last_qpos = chk(last_qpos, (B, self.opt_dof), torch.float32, "last_qpos")
+        nf = len(self.idx_pin2fixed)
+        if nf:
+            if fixed_qpos is None:
+                raise ValueError(f"Optimizer has {nf} joints but no fixed_qpos is given")
+            io.fixed_qpos = chk(fixed_qpos, (B, nf), torch.float32, "fixed_qpos")
+
+    # ---------------------------------------------------------------- objective evaluation
+    def objective_batch(self, qpos, ref_value=None, fixed_qpos=None, last_qpos=None, *, keypoints=None, projected=None,
+                        raw_hand=None, loss_out=None, cost_out=None, grad_out=None, want_grad=True, stream=None):
+        """The objective at B given joint vectors, one launch (`dexr_eval_objective`), no solve.  Tensors as for
+        `retarget_batch`; `qpos` [B,opt_dof] is the point of evaluation, used as given (no clipping to the limits); `last_qpos`
+        [B,opt_dof] is the anchor of the norm_delta term (None: no regulariser); `projected` [B,len_proj] uint8 DexPilot flags
+        are read and updated as by a solve on the same targets (None: every frame starts unprojected).
+        Returns (loss [B], cost [B], grad [B,opt_dof] or None), CUDA tensors on this optimizer's device:
+          loss = L(x), the value of the reference's objective closure;
+          cost = L(x) + norm_delta |x - last_qpos|^2, what `retarget_batch(cost_out=...)` reports at its answer;
+          grad = d cost / dx, the reference closure's `grad` (with want_grad; a given grad_out implies it).
+        Nothing is synchronised."""
+        import torch
+
+        eng = self.engine()
+        dev = torch.device("cuda", eng.device)
+        chk = _tensor_check(dev)
+        B = qpos.shape[0]
+        io = N.DexrEval()
+        io.qpos = chk(qpos, (B, self.opt_dof), torch.float32, "qpos")
+        self._batch_targets(io, chk, B, ref_value, keypoints, fixed_qpos, last_qpos=last_qpos)
+        if projected is not None:
+            io.projected = chk(projected, (B, self._objective_spec().len_proj), torch.uint8, "projected")
+        if raw_hand is not None and keypoints is None:
+            raise ValueError("raw_hand needs `keypoints` (raw landmarks), not ref_value")
+        loss_out = torch.empty((B,), dtype=torch.float32, device=dev) if loss_out is None else loss_out
+        cost_out = torch.empty((B,), dtype=torch.float32, device=dev) if cost_out is None else cost_out
+        io.loss_out = chk(loss_out, (B,), torch.float32, "loss_out")
+        io.cost_out = chk(cost_out, (B,), torch.float32, "cost_out")
+        if want_grad or grad_out is not None:
+            grad_out = torch.empty((B, self.opt_dof), dtype=torch.float32, device=dev) if grad_out is None else grad_out
+            io.grad_out = chk(grad_out, (B, self.opt_dof), torch.float32, "grad_out")
+        p = self.params(raw_hand=raw_hand)
+        s = stream if stream is not None else torch.cuda.current_stream(dev)
+        N.check(eng.lib.dexr_eval_objective(eng.handle, C.byref(p), C.byref(io), B, C.c_void_p(s.cuda_stream)),
+                "dexr_eval_objective")
+        return loss_out, cost_out, grad_out
+
+    def _objective_flags(self):
+        """Hysteresis state an objective closure starts from (DexPilot only)."""
+        return None
+
+    def _set_objective_flags(self, flags):
+        pass
+
+    def get_objective_function(self, ref_value, fixed_qpos, last_qpos):
+        """The reference's closure (optimizer.py:104-108): `objective(x, grad) -> float` returns L(x) and, when grad.size > 0,
+        fills grad[:] with the gradient of L(x) + norm_delta |x - last_qpos|^2 -- what nlopt is handed.  Every call is one
+        one-frame `dexr_eval_objective` launch and a synchronise, on device buffers allocated here once."""
+        import torch
+
+        if len(fixed_qpos) != len(self.idx_pin2fixed):
+            raise ValueError(
+                f"Optimizer has {len(self.idx_pin2fixed)} joints but non_target_qpos {fixed_qpos} is given"
+            )
+        dev = torch.device("cuda", self.engine().device)
+        n, nf = self.opt_dof, len(self.idx_pin2fixed)
+
+        def on_dev(a, shape):
+            return torch.as_tensor(np.asarray(a, dtype=np.float32).reshape(shape)).to(dev)
+
+        ref = on_dev(ref_value, (1, self.num_residuals, 3))
+        fixed = on_dev(fixed_qpos, (1, nf)) if nf else None
+        last = on_dev(last_qpos, (1, n))  # float32 like the reference's last_qpos (optimizer.py:92-94)
+        x_dev = torch.empty((1, n), dtype=torch.float32, device=dev)
+        out = torch.empty((2 + n,), dtype=torch.float32, device=dev)  # loss, cost, grad: read back with one copy
+        loss_t, cost_t, grad_t = out[0:1], out[1:2], out[2:].view(1, n)
+        flags = self._objective_flags()
+        proj = None
+        if flags is not None:
+            # DexPilot updates its hysteresis state when the closure is made (optimizer.py:466-476).  Every call then
+            # evaluates with these flags, updating them again: for fixed targets the update is idempotent (applied to its
+            # own output it gives the same flags and weights), so every call sees the same objective.
+            proj = torch.as_tensor(np.asarray(flags, dtype=np.uint8).reshape(1, -1)).to(dev)
+            self.objective_batch(last, ref, fixed, last, projected=proj, loss_out=loss_t, cost_out=cost_t, want_grad=False)
+            self._set_objective_flags(proj[0].cpu().numpy().astype(bool))
+
+        def objective(x: np.ndarray, grad: np.ndarray) -> float:
+            x_dev.copy_(torch.from_numpy(np.asarray(x, dtype=np.float32).reshape(1, n)))
+            want = grad.size > 0
+            self.objective_batch(x_dev, ref, fixed, last, projected=proj, loss_out=loss_t, cost_out=cost_t,
+                                 grad_out=grad_t if want else None, want_grad=want)
+            res = out.cpu().numpy()  # (synchronises)
+            if want:
+                grad[:] = res[2:]
+            return float(res[0])
+
+        return objective
+
+
+def _tensor_check(dev):
+    """chk(tensor, shape, dtype, name) -> data pointer, or ValueError unless the tensor is contiguous, of that dtype and
+    shape, on `dev`."""
+
+    def chk(t, shape, dtype, name):
+        if t.device != dev or t.dtype != dtype or not t.is_contiguous() or tuple(t.shape) != tuple(shape):
+            raise ValueError(f"{name}: expected contiguous {dtype} tensor of shape {tuple(shape)} on {dev}, "
+                             f"got {t.dtype} {tuple(t.shape)} on {t.device}")
+        return t.data_ptr()
+
+    return chk
 
 
 def retarget_batch_mixed(jobs, stream=None):
@@ -566,6 +673,12 @@ class DexPilotOptimizer(Optimizer):
     def _loss_params(self, p):
         p.huber_delta, p.norm_delta, p.scaling = self.huber_delta, self.norm_delta, self.scaling
         p.project_dist, p.escape_dist, p.eta1, p.eta2 = self.project_dist, self.escape_dist, self.eta1, self.eta2
+
+    def _objective_flags(self):
+        return self.projected
+
+    def _set_objective_flags(self, flags):
+        self.projected = flags
 
     def retarget(self, ref_value, fixed_qpos, last_qpos, damping=None):
         if len(fixed_qpos) != len(self.idx_pin2fixed):

@@ -260,6 +260,30 @@ int dexr_preprocess_keypoints(const float* raw, float* out, float* wrist_rot_out
 /* Launch geometry of the last call on this handle (diagnostics / bench reporting). */
 int dexr_get_launch_info(const dexr_robot_t* robot, dexr_launch_info_t* out);
 
+/* ---------------------------------------------------------------------------------------------
+ * Objective evaluation: the value and gradient of the retargeting objective at GIVEN joint vectors, no solve.  Replaces B
+ * calls of the closure returned by Optimizer.get_objective_function (optimizer.py:104-108, implemented at :138-200,
+ * :241-306, :456-577): scoring recorded or foreign joint trajectories against human keypoints, and the objective as a
+ * training loss.  Targets are prepared exactly as by dexr_solve_frames (keypoint gather, params.preprocess, scaling,
+ * DexPilot flags and weights); the call reads the loss fields of `params` and `preprocess`, and ignores tol, lambda0,
+ * max_iters, clip_init and lp_alpha.  Asynchronous on `cuda_stream`, allocates nothing; num_frames == 0 does nothing.
+ * A frame with a non-finite input gets non-finite outputs; no other frame changes.  All pointers are DEVICE pointers.
+ * ------------------------------------------------------------------------------------------- */
+typedef struct dexr_eval {
+  const float* keypoints;  /* [B,21,3] or NULL  } exactly one of the two; raw landmarks with params.preprocess     */
+  const float* ref_value;  /* [B,m,3]  or NULL  }                                                                     */
+  const float* fixed_qpos; /* [B,n_fixed] or NULL when n_fixed == 0                                                   */
+  const float* qpos;       /* [B,n_var] the point of evaluation, target_joint_names order, used as given (no clipping) */
+  const float* last_qpos;  /* [B,n_var] anchor of the norm_delta term, or NULL: no regulariser                        */
+  uint8_t* projected;      /* [B,len_proj] DexPilot flags, read and updated as by dexr_solve_frames; NULL: start false */
+  float* loss_out;         /* [B] or NULL: L(x), what the reference's closure returns                                 */
+  float* cost_out;         /* [B] or NULL: L(x) + norm_delta |x - last|^2, the quantity dexr_frames_t.cost_out reports */
+  float* grad_out;         /* [B,n_var] or NULL: gradient of cost_out = the reference closure's grad                   */
+} dexr_eval_t;
+size_t dexr_eval_sizeof(void);
+int dexr_eval_objective(const dexr_robot_t* robot, const dexr_params_t* params, const dexr_eval_t* io,
+                        int64_t num_frames, void* cuda_stream);
+
 #ifdef __cplusplus
 }
 #endif
