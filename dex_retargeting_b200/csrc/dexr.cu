@@ -121,7 +121,7 @@ __device__ __forceinline__ void frames_group(const FrameArgs& a, int first_tile)
     constexpr int GPW = 32 / G;
     const int gid = warp * GPW + (lane / G);
     Solver<G, BW> sv;
-    sv.init(a.table, a.dm, (uint32_t)(a.scratch_off + gid * Scratch<G>::kFloats * 4), a.prm, lane);
+    sv.init(a.table, a.dm, (uint32_t)(a.scratch_off + gid * Scratch<G, BW>::kFloats * 4), a.prm, lane);
 
     int it = 0;
     for (int tile = first_tile; tile < a.ntiles; tile += gridDim.x, ++it) {
@@ -220,8 +220,8 @@ __global__ void __launch_bounds__(NW * 32, 1) dexr_sequences_kernel(const SeqArg
   const int lane = threadIdx.x & 31;
   const int gid = warp * GPW + (lane / G);               // scratch slot of this group of lanes
   const int slots_per_cta = NW * a.spw;
-  const uint32_t scratch_off = (uint32_t)(a.scratch_off + gid * Scratch<G>::kStreamFloats * 4);
-  float* kpbuf = reinterpret_cast<float*>(smem + scratch_off) + Scratch<G>::kFloats;  // 63 floats: current keypoints
+  const uint32_t scratch_off = (uint32_t)(a.scratch_off + gid * Scratch<G, BW>::kStreamFloats * 4);
+  float* kpbuf = reinterpret_cast<float*>(smem + scratch_off) + Scratch<G, BW>::kFloats;  // 63 floats: current keypoints
   const int slot = a.spw == GPW ? gid : warp;            // which of the CTA's stream slots this group serves
   const bool first = (lane / G) == 0;
   const bool owner = a.spw == GPW || first;              // the group that reads and writes the stream's state
@@ -623,7 +623,7 @@ static bool arrow_enabled() {
 
 // Fill the kernel arguments of one robot group: tile size, ring layout, dynamic shared memory.  `slots` = CTAs the tiles are
 // spread over.  Returns the dynamic shared memory the group needs.
-template <int G, int NCW>
+template <int G, int BW, int NCW>
 static int fill_frame_args(const dexr_robot* r, const dexr_params_t* prm, const dexr_frames_t* io, long long B, int slots, FrameArgs& a, int tile = 0) {
   const dexr_table_t& t = r->host;
   a = FrameArgs{};
@@ -662,14 +662,14 @@ static int fill_frame_args(const dexr_robot* r, const dexr_params_t* prm, const 
   a.bar_off = a.ring_off + 2 * a.stage_bytes;
   a.scratch_off = round_up(a.bar_off + 4 * 8 + 2 * 4, 16);
   constexpr int GPW = 32 / G;
-  return a.scratch_off + NCW * GPW * Scratch<G>::kFloats * 4;
+  return a.scratch_off + NCW * GPW * Scratch<G, BW>::kFloats * 4;
 }
 
 template <int G, int BW, int NCW>
 static int launch_frames(dexr_robot* r, const dexr_params_t* prm, const dexr_frames_t* io, long long B, cudaStream_t stream, int slots, int tile) {
   FrameArgs a;
   if (slots <= 0) slots = r->num_sms;  // one persistent CTA per SM; a mixed launch passes its own CTA count and tile size
-  const int smem = fill_frame_args<G, NCW>(r, prm, io, B, slots, a, tile);
+  const int smem = fill_frame_args<G, BW, NCW>(r, prm, io, B, slots, a, tile);
   auto kern = dexr_frames_kernel<G, BW, NCW>;
   CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
   const int grid = std::min(a.ntiles, slots);
@@ -682,20 +682,24 @@ static int launch_frames(dexr_robot* r, const dexr_params_t* prm, const dexr_fra
   return 0;
 }
 
-// Consumer warps per CTA for each solver kind (index = solver_kind()): the register file (64 K x 32 bit per SM, one CTA per
-// SM) gives 128 registers per thread at 15 + 1 warps, 144 at 13 + 1, 168 at 11 + 1.  Measured on H100 SXM (400 W, 65 536
-// frames per launch, 16 | 14 | 12 warps, ms): every solver kind is fastest with 16 warps despite the spills at 128
-// registers -- Allegro vector (block) 0.265 | 0.290 | 0.305, LEAP DexPilot (dense 16) 1.77 | 1.86 | 1.80, Ability (dense 16,
-// mimic) 1.52 | 1.67 | 1.75, Shadow position (arrow) 3.21 | 3.37 | 3.45, SVH (dense 32) 4.34 | 4.75 | 4.80.
-// DEXR_FRAMES_WARPS="a,b,c,d" (16 | 14 | 12 per kind) overrides for A/B runs.
+// Consumer warps per CTA for each solver kind (index = solver_kind()), counted with the producer.  One CTA per SM; ptxas splits
+// the 64 K x 32-bit register file over the SM's four sub-partitions (16 K registers each, warps dealt round-robin), so the
+// caps are 168 registers per thread at 12 warps, 128 at 13-16, 96 at 17-20, 80 at 21-24 and 72 at 25-28: a count between
+// two steps buys no registers.  Measured on H100 SXM (400 W, 65 536 frames per launch, 16 | 14 | 12 warps, ms): every dense
+// and arrow kind is fastest with 16 warps despite the spills at 128 registers -- LEAP DexPilot (dense 16) 1.77 | 1.86 | 1.80,
+// Ability (dense 16, mimic) 1.52 | 1.67 | 1.75, Shadow position (arrow) 3.21 | 3.37 | 3.45, SVH (dense 32) 4.34 | 4.75 | 4.80.
+// The block-diagonal solver needs 119 registers and runs fastest with 24 warps at 80 (sweep: DESIGN.md 3.1).
+// DEXR_FRAMES_WARPS="a,b,c,d" overrides for A/B runs: block 16 | 20 | 24 | 28, the other kinds 16 | 14 | 12.
 static const int* frames_warps() {
-  static int w[4] = {16, 16, 16, 16};
+  static int w[4] = {24, 16, 16, 16};
   static const bool init = [] {
     if (const char* e = getenv("DEXR_FRAMES_WARPS")) {
       int v[4];
-      if (sscanf(e, "%d,%d,%d,%d", &v[0], &v[1], &v[2], &v[3]) == 4)
-        for (int i = 0; i < 4; ++i)
+      if (sscanf(e, "%d,%d,%d,%d", &v[0], &v[1], &v[2], &v[3]) == 4) {
+        if (v[0] == 16 || v[0] == 20 || v[0] == 24 || v[0] == 28) w[0] = v[0];
+        for (int i = 1; i < 4; ++i)
           if (v[i] == 16 || v[i] == 14 || v[i] == 12) w[i] = v[i];
+      }
     }
     return true;
   }();
@@ -705,8 +709,14 @@ static const int* frames_warps() {
 
 template <int G, int BW>
 static int launch_frames_warps(int warps, dexr_robot* r, const dexr_params_t* prm, const dexr_frames_t* io, long long B, cudaStream_t stream, int slots, int tile) {
-  if (warps == 12) return launch_frames<G, BW, 11>(r, prm, io, B, stream, slots, tile);
-  if (warps == 14) return launch_frames<G, BW, 13>(r, prm, io, B, stream, slots, tile);
+  if constexpr (BW > 0) {
+    if (warps == 20) return launch_frames<G, BW, 19>(r, prm, io, B, stream, slots, tile);
+    if (warps == 24) return launch_frames<G, BW, 23>(r, prm, io, B, stream, slots, tile);
+    if (warps == 28) return launch_frames<G, BW, 27>(r, prm, io, B, stream, slots, tile);
+  } else {
+    if (warps == 12) return launch_frames<G, BW, 11>(r, prm, io, B, stream, slots, tile);
+    if (warps == 14) return launch_frames<G, BW, 13>(r, prm, io, B, stream, slots, tile);
+  }
   return launch_frames<G, BW, 15>(r, prm, io, B, stream, slots, tile);
 }
 
@@ -823,8 +833,9 @@ extern "C" int dexr_solve_frames_multi(const dexr_group_t* groups, int32_t num_g
     if (r->device != device) return fail(DEXR_E_INVALID, "group %d lives on device %d, group 0 on device %d: one launch, one device", i, r->device, device);
     const SolverKind k = solver_kind(r->host, arrow_enabled());
     FrameArgs& a = m.g[m.n_groups];
-    const int need = kind_lanes(k) == 16 ? fill_frame_args<16, NCW>(r, g.params, &g.io, g.num_frames, sms, a)
-                                         : fill_frame_args<32, NCW>(r, g.params, &g.io, g.num_frames, sms, a);
+    const int need = with_solver(k, [&](auto s) {
+      return fill_frame_args<decltype(s)::G, decltype(s)::BW, NCW>(r, g.params, &g.io, g.num_frames, sms, a);
+    });
     smem = std::max(smem, need);
     m.kind[m.n_groups++] = k;
     tiles += a.ntiles;
@@ -958,7 +969,7 @@ static int launch_sequences(dexr_robot* r, const dexr_params_t* prm, const dexr_
   a.scratch_off = round_up((int)sizeof(SharedTable), 16);
   constexpr int GPW = 32 / G;
   const int groups = kSeqNW * GPW;
-  const int smem = a.scratch_off + groups * Scratch<G>::kStreamFloats * 4;
+  const int smem = a.scratch_off + groups * Scratch<G, BW>::kStreamFloats * 4;
   auto kern = dexr_sequences_kernel<G, BW, kSeqNW>;
   CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
   // A stream is serial in time and latency bound, so streams are spread over as many warps and SMs as there are: while one

@@ -164,6 +164,22 @@ __device__ __forceinline__ float fast_rcp(float x) {
 #endif
 }
 
+// v, passed through an empty asm the compiler cannot look into or move: what is derived from the result is computed where it
+// is used instead of being hoisted out of the frame loop as a loop invariant and held in a register through every frame.
+// No instruction is emitted.
+__device__ __forceinline__ uint32_t opaque(uint32_t v) {
+#ifndef DEXR_HOST_EMULATION
+  asm volatile("" : "+r"(v));
+#endif
+  return v;
+}
+__device__ __forceinline__ long long opaque(long long v) {
+#ifndef DEXR_HOST_EMULATION
+  asm volatile("" : "+l"(v));
+#endif
+  return v;
+}
+
 __device__ __forceinline__ float huber_val(float d, float beta, float inv_beta) {
   return d < beta ? 0.5f * d * d * inv_beta : d - 0.5f * beta;
 }
@@ -332,16 +348,20 @@ __device__ inline void load_shared_table(SharedTable& st, const dexr_table_t* __
 // ------------------------------------------------------------------------------------------------
 // per-group scratch in shared memory (floats)
 // ------------------------------------------------------------------------------------------------
-template <int G>
+// BW: the Solver<G, BW> instantiation the group runs.  Block mode (BW > 0) backs up and transposes only the BW-column row
+// segments its lanes hold (2.3 KB instead of 3.9 KB per 16-lane group: room for more consumer warps next to the ring);
+// dense mode needs all NP rows (and the mimic-fold temporaries), arrow mode keeps its Schur matrix in the backup area.
+template <int G, int BW = 0>
 struct Scratch {
   static constexpr int NP = G;
+  static constexpr int kRows = BW > 0 ? BW : NP;                // rows of the backup and of the transposed factor
   static constexpr int kFr = 0;                                 // [MAX_RES][4] target xyz, weight c_k
   static constexpr int kLp = kFr + DEXR_MAX_RES * 4;            // [2][MAX_LINKS][4] link positions
   static constexpr int kU = kLp + 2 * DEXR_MAX_LINKS * 4;       // jbuf[2][3][NP] (aliased by the 2 Cholesky row buffers) + at: 2 x [NP + NP/4] float4
   static constexpr int kUSize = 16 * NP;
-  static constexpr int kHb = kU + kUSize;                       // [NP][NP]   Hessian backup, column per lane
-  static constexpr int kLcol = kHb + NP * NP;                   // [NP][NP+1] L^T rows, conflict-free column reads (also mimic-fold temp)
-  static constexpr int kFloats = ((kLcol + NP * (NP + 1) + 3) / 4) * 4;
+  static constexpr int kHb = kU + kUSize;                       // [kRows][NP]   Hessian backup, column per lane
+  static constexpr int kLcol = kHb + kRows * NP;                // [kRows][NP+1] L^T rows, conflict-free column reads (also mimic-fold temp)
+  static constexpr int kFloats = ((kLcol + kRows * (NP + 1) + 3) / 4) * 4;
   static constexpr int kStreamFloats = kFloats + 64;  // sequences: followed by the current frame's 63 keypoint floats
 };
 
@@ -370,7 +390,7 @@ struct Solver {
   static_assert(BW >= 0 || G == 32, "arrow mode is a 32-lane layout");
   static constexpr bool AR = BW < 0;
   static constexpr int HN = (BW == 0) ? G : (AR ? 16 : BW);  // Hessian row segment held per lane
-  using SC = Scratch<G>;
+  using SC = Scratch<G, BW>;
 
   // ---- lane constants kept in registers (the 3x4 joint placement lives in shared memory) ----
   float lo, hi, mmult, moff;
@@ -412,6 +432,19 @@ struct Solver {
     mmult = tb->mimic_mult[c]; moff = tb->mimic_off[c];
     jtype = tb->jtype[c]; var = tb->var_index[c]; msrc = tb->mimic_src[c];
     jump = tb->jump[c]; anc = tb->anc_mask[c]; desc = tb->desc_mask[c];
+  }
+
+  // The block-diagonal frames kernel runs 24 warps per SM at 80 registers (dexr.cu, frames_warps()).  There the lane's integer
+  // constants (lane index, scratch offset, ancestor / descendant masks, variable index, joint type) are passed through opaque()
+  // at the top of every iteration, trial and fallback pass and after the trial FK, so that the shared-memory addresses, masks
+  // and predicates derived from them are recomputed where they are used (a few integer instructions) instead of being held
+  // in registers -- or spilled -- from one use to the next.  Other instantiations are unchanged.
+  __device__ __forceinline__ void refresh() {
+    if constexpr (BW > 0) {
+      l = (int)opaque((uint32_t)l); lane = (int)opaque((uint32_t)lane);
+      sc_off = opaque(sc_off); anc = opaque(anc); desc = opaque(desc);
+      var = (int)opaque((uint32_t)var); jtype = (int)opaque((uint32_t)jtype);
+    }
   }
 
   __device__ __forceinline__ float* scf() const { return reinterpret_cast<float*>(dsmem + sc_off); }
@@ -489,12 +522,13 @@ struct Solver {
   }
 
   // World axis of this lane's joint from its world rotation (the Jacobian column direction, robot_wrapper.py:93-95).
-  __device__ __forceinline__ void set_world_axis(const float* Rw) {
+  __device__ __forceinline__ void world_axis(const float* Rw, float* ax) const {
     const float ax0 = ST().lane_c[6][l].w, ax1 = ST().lane_c[7][l].w, ax2 = ST().lane_c[8][l].w;
-    a[0] = fmaf(Rw[0], ax0, fmaf(Rw[1], ax1, Rw[2] * ax2));
-    a[1] = fmaf(Rw[3], ax0, fmaf(Rw[4], ax1, Rw[5] * ax2));
-    a[2] = fmaf(Rw[6], ax0, fmaf(Rw[7], ax1, Rw[8] * ax2));
+    ax[0] = fmaf(Rw[0], ax0, fmaf(Rw[1], ax1, Rw[2] * ax2));
+    ax[1] = fmaf(Rw[3], ax0, fmaf(Rw[4], ax1, Rw[5] * ax2));
+    ax[2] = fmaf(Rw[6], ax0, fmaf(Rw[7], ax1, Rw[8] * ax2));
   }
+  __device__ __forceinline__ void set_world_axis(const float* Rw) { world_axis(Rw, a); }
 
   // Link origins (robot_wrapper.py:85-87 [updateFramePlacement]) -> shared buffer b.  Each lane places the links
   // that ride on its joint (normally one); links fixed to the world are written once per frame (prelude).
@@ -728,6 +762,7 @@ struct Solver {
     }
 
     while (gany<32>(!done, lane)) {
+      refresh();
       // ======================= gradient + exact Hessian at x ===========================
       float H[HN];
 #pragma unroll
@@ -990,10 +1025,13 @@ struct Solver {
       // ======================= damped Newton trials ====================================
       bool accepted = done;
       float acc_step = 0.f;
-      float Rn[9], pn[3];
+      float Rn[9], pn[3], an[3];
       for (int trial = 0; trial < kMaxTrials; ++trial) {
         if (!gany<32>(!accepted, lane)) break;
-        if (trial > 0) {
+        refresh();
+        // block mode reads H back from the backup on the first trial too (the same values) instead of holding it in registers
+        // through the active-set and trust bookkeeping
+        if (trial > 0 || BW > 0) {
 #pragma unroll
           for (int i = 0; i < HN; ++i) H[i] = hbuf[i * NP + l];
         }
@@ -1197,6 +1235,7 @@ struct Solver {
         {
           const bool drop = bad && !accepted && curv_in;
           if (gany<32>(drop, lane)) {
+            refresh();
             const float4 a_self = at_a(l);          // (rev ? a : 0), t of this lane, as stored when H was built
             const float4 t_self = at_t(l);
 #pragma unroll
@@ -1237,7 +1276,11 @@ struct Solver {
         const float pred = 0.5f * gsum<G>(dx * fmaf(lam * D, dx, -g));
         const float qn = compose_q(xn);
         fk(qn, Rn, pn);
+        refresh();
         write_links(Rn, pn, cur ^ 1);
+        // block mode: the trial point's world axis right away, so that its 3x3 rotation is dead through cost() and the
+        // acceptance test (6 live registers fewer; the same operations, also on a rejected trial)
+        if constexpr (BW > 0) world_axis(Rn, an);
         __syncwarp();
         cost(cur ^ 1, xn);
         // F(xn) - F(x) summed term by term: every lane differences its own residual / regulariser term (nearby numbers: the
@@ -1259,7 +1302,12 @@ struct Solver {
             x = xn; q = qn; F = Fn;
             Fnz = cost_nz;
             Fl = cost_lane;
-            set_world_axis(Rn);
+            if constexpr (BW > 0) {
+#pragma unroll
+              for (int i = 0; i < 3; ++i) a[i] = an[i];
+            } else {
+              set_world_axis(Rn);
+            }
 #pragma unroll
             for (int i = 0; i < 3; ++i) p[i] = pn[i];
             cur ^= 1;
@@ -1357,6 +1405,7 @@ __device__ __forceinline__ void solve_frame(Solver<G, BW>& sv, const FrameInputs
                                             long long f, bool active) {
   sv.lam_carry = io.damping_io ? io.damping_io[f] : 0.f;  // (every lane of the group reads the frame's word)
   const int status = sv.solve(in, active);
+  if constexpr (BW > 0) f = opaque(f);  // (the output addresses are formed here, not held through the solve: see Solver::refresh)
   if (active) {
     if (sv.var >= 0) io.qpos_out[f * dm.n_var + sv.var] = sv.x;
     if (io.robot_qpos_out && sv.l < dm.dof) io.robot_qpos_out[f * dm.dof + sv.l] = sv.q;

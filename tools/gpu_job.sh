@@ -137,7 +137,7 @@ PY
   done
 fi
 if want warps; then
-  for cfg in 16,16,16,16 14,14,14,14 12,12,12,12; do
+  for cfg in 16,16,16,16 20,14,14,14 24,12,12,12; do  # (block diagonal: 16 | 20 | 24, the other kinds 16 | 14 | 12)
     DEXR_FRAMES_WARPS=$cfg python - <<'PY'
 import os, sys, torch
 sys.path.insert(0, "tools")
