@@ -376,6 +376,71 @@ struct FrameInputs {
   uint8_t* projected;  // len_proj flags (global) or nullptr
 };
 
+// The integer and boolean bookkeeping of Solver::solve (group-uniform).  Packed (the 16-lane block-diagonal solver, whose
+// frames kernel runs at 80 registers): two words instead of eleven registers carried through every phase of an iteration.
+//   w0: bits 0-15 iterations, 16-22 rejected trials (saturated at 127), 23-25 the status flags, 26 done, 27 exact,
+//       28 recheck, 29 trust_prev, 30-31 stall (saturated at 3: only `stall >= 2` is read)
+//   w1: bits 0-15 the free-variable mask of the previous iteration, 16-17 rechecks (at most 3)
+// w0 & 0x3ffffff is the status word (dexr.h).  Unpacked: one variable each.
+template <bool P>
+struct Bookkeeping {
+  static constexpr uint32_t kDone = 1u << 26, kExact = 1u << 27, kRecheck = 1u << 28, kTrust = 1u << 29;
+  uint32_t w0 = kExact, w1 = 0;
+  int iters_ = 0, rejects_ = 0, rechecks_ = 0, stall_ = 0, status_ = 0;
+  unsigned last_fmask_ = 0u;
+  bool done_ = false, exact_ = true, recheck_ = false, trust_ = false;
+
+  __device__ __forceinline__ bool get(uint32_t bit, bool v) const { return P ? (w0 & bit) != 0u : v; }
+  __device__ __forceinline__ void put(uint32_t bit, bool& v, bool x) {
+    if constexpr (P) w0 = x ? (w0 | bit) : (w0 & ~bit);
+    else v = x;
+  }
+  __device__ __forceinline__ bool done() const { return get(kDone, done_); }
+  __device__ __forceinline__ void set_done(bool x) { put(kDone, done_, x); }
+  __device__ __forceinline__ bool exact() const { return get(kExact, exact_); }
+  __device__ __forceinline__ void set_exact(bool x) { put(kExact, exact_, x); }
+  __device__ __forceinline__ bool recheck() const { return get(kRecheck, recheck_); }
+  __device__ __forceinline__ void set_recheck(bool x) { put(kRecheck, recheck_, x); }
+  __device__ __forceinline__ bool trust_prev() const { return get(kTrust, trust_); }
+  __device__ __forceinline__ void set_trust_prev(bool x) { put(kTrust, trust_, x); }
+  __device__ __forceinline__ void flag(int s) {
+    if constexpr (P) w0 |= (uint32_t)s;
+    else status_ |= s;
+  }
+  __device__ __forceinline__ int iters() const { return P ? (int)(w0 & 0xffffu) : iters_; }
+  __device__ __forceinline__ void inc_iters() {  // (max_iters <= 65535: the field does not wrap)
+    if constexpr (P) ++w0;
+    else ++iters_;
+  }
+  __device__ __forceinline__ void inc_rejects() {
+    if constexpr (P) { if ((w0 & (0x7fu << 16)) != (0x7fu << 16)) w0 += 1u << 16; }
+    else ++rejects_;
+  }
+  __device__ __forceinline__ int stall() const { return P ? (int)(w0 >> 30) : stall_; }
+  __device__ __forceinline__ void clear_stall() {
+    if constexpr (P) w0 &= ~(3u << 30);
+    else stall_ = 0;
+  }
+  __device__ __forceinline__ void inc_stall() {
+    if constexpr (P) { if ((w0 >> 30) != 3u) w0 += 1u << 30; }
+    else ++stall_;
+  }
+  __device__ __forceinline__ unsigned last_fmask() const { return P ? (w1 & 0xffffu) : last_fmask_; }
+  __device__ __forceinline__ void set_last_fmask(unsigned m) {
+    if constexpr (P) w1 = (w1 & ~0xffffu) | m;
+    else last_fmask_ = m;
+  }
+  __device__ __forceinline__ int inc_rechecks() {  // ++rechecks
+    if constexpr (P) { w1 += 1u << 16; return (int)(w1 >> 16); }
+    else return ++rechecks_;
+  }
+  // the status word: flags, iterations and rejected trials (saturated at 127)
+  __device__ __forceinline__ int status() const {
+    if constexpr (P) return (int)(w0 & 0x3ffffffu);
+    else return status_ | ((iters_ & 0xffff) | ((rejects_ > 127 ? 127 : rejects_) << 16));
+  }
+};
+
 template <int G, int BW = 0>
 struct Solver {
   static constexpr int NP = G;
@@ -432,18 +497,30 @@ struct Solver {
     mmult = tb->mimic_mult[c]; moff = tb->mimic_off[c];
     jtype = tb->jtype[c]; var = tb->var_index[c]; msrc = tb->mimic_src[c];
     jump = tb->jump[c]; anc = tb->anc_mask[c]; desc = tb->desc_mask[c];
+    if constexpr (BW > 0) {
+      static_assert(BW <= 0 || G == 16, "the packed lane constants hold 16-lane masks");
+      lane_pk = (uint32_t)lane | ((uint32_t)(var + 1) << 5) | ((jtype != 0 ? 1u : 0u) << 10) | ((sc_off >> 4) << 12);
+      mask_pk = (anc & 0xffffu) | (desc << 16);
+    }
   }
 
   // The block-diagonal frames kernel runs 24 warps per SM at 80 registers (dexr.cu, frames_warps()).  There the lane's integer
-  // constants (lane index, scratch offset, ancestor / descendant masks, variable index, joint type) are passed through opaque()
-  // at the top of every iteration, trial and fallback pass and after the trial FK, so that the shared-memory addresses, masks
-  // and predicates derived from them are recomputed where they are used (a few integer instructions) instead of being held
-  // in registers -- or spilled -- from one use to the next.  Other instantiations are unchanged.
+  // constants (lane index, scratch offset, ancestor / descendant masks, variable index, joint type) are kept packed in two
+  // words, lane_pk and mask_pk, which pass through opaque() at the top of every frame, iteration, trial and fallback pass
+  // and after the trial FK; the members are unpacked from them there.  So two registers carry the constants from one phase
+  // to the next, and the shared-memory addresses, masks and predicates derived from them are recomputed where they are used
+  // (a few integer instructions) instead of being held in registers -- or spilled -- from one use to the next.
+  //   lane_pk: bits 0-4 lane, 5-9 var + 1, 10 jtype != 0 (only `jtype == 0` is read), 12-31 sc_off / 16
+  //   mask_pk: bits 0-15 anc, 16-31 desc
+  // Other instantiations are unchanged.
+  uint32_t lane_pk = 0u, mask_pk = 0u;
   __device__ __forceinline__ void refresh() {
     if constexpr (BW > 0) {
-      l = (int)opaque((uint32_t)l); lane = (int)opaque((uint32_t)lane);
-      sc_off = opaque(sc_off); anc = opaque(anc); desc = opaque(desc);
-      var = (int)opaque((uint32_t)var); jtype = (int)opaque((uint32_t)jtype);
+      lane_pk = opaque(lane_pk); mask_pk = opaque(mask_pk);
+      lane = (int)(lane_pk & 31u); l = lane & (G - 1);
+      var = (int)((lane_pk >> 5) & 31u) - 1; jtype = (int)((lane_pk >> 10) & 1u);
+      sc_off = (lane_pk >> 12) << 4;
+      anc = mask_pk & 0xffffu; desc = mask_pk >> 16;
     }
   }
 
@@ -682,7 +759,8 @@ struct Solver {
     const int dof = dm.dof;
     const float nd = prm.norm_delta;
     const float beta = prm.huber_delta;
-    int status = 0;
+    Bookkeeping<(BW > 0 && G == 16)> bk;
+    refresh();
 
     // ---- prelude: warm start, anchor, fixed joints (optimizer.py:138-141, seq_retarget.py:115-121)
     float xin = 0.f;
@@ -698,7 +776,7 @@ struct Solver {
     finite = !gany<G>(!finite, lane) && ok_in;
     __syncwarp();
     if (!finite) {
-      status |= DEXR_STATUS_NONFINITE;
+      bk.flag(DEXR_STATUS_NONFINITE);
       x = x0;
       if (!isfinite(x)) x = 0.f;
       if (!isfinite(qfix)) qfix = 0.f;
@@ -721,17 +799,12 @@ struct Solver {
 
     float lam = lam_carry > 0.f ? lam_carry : prm.lambda0;  // (kCarry)
     lam_carry = prm.lambda0;
-    int iters = 0, rejects = 0;
-    bool done = !active;
+    bk.set_done(!active);
     // Curvature model (group-uniform): `exact` = use the true second derivative of the norm-Huber loss
     // (radial direction has zero curvature beyond beta); otherwise its quadratic majoriser 1/d * I, which
     // is positive semi-definite and globally safer.  Optimistic start, demoted after a large or failed step.
-    bool exact = true;
     // A tiny accepted step ends the frame -- unless some variable is held at a bound: then the gradient is
     // re-evaluated once more, and the frame ends only if the same set stays active (KKT on the bounds).
-    bool recheck = false;
-    int rechecks = 0;
-    unsigned last_fmask = 0u;
     // Steps whose predicted decrease is below what fp32 resolves in F are taken on trust; whether they were any good is read
     // off the GRADIENT one iteration later (it is computed directly, not by differencing F, and resolves far below the noise
     // of F).  A smaller gradient max-norm keeps the step and relaxes the damping like a verified decrease would.  A gradient
@@ -742,8 +815,6 @@ struct Solver {
     // max_iters).  Two reverts in a row mean the KKT residual sits at its fp32 floor: the frame ends at the best point.
     float gn_prev = 0.f, x_prev = 0.f;
     float s_prev = 0.f;  // the previous iteration's accepted step when that was a first-trial Newton step, else 0
-    bool trust_prev = false;
-    int stall = 0;
 
     // ---- arrow mode: this lane's finger window (see the Solver comment); loop invariant ----
     int ar_t = 0, ar_fb = 0, ar_fw = 0, ar_maxw = 0, ar_fo = 0;
@@ -761,7 +832,7 @@ struct Solver {
       ar_maxw = (int)gmax<G>((float)ar_fw);
     }
 
-    while (gany<32>(!done, lane)) {
+    while (gany<32>(!bk.done(), lane)) {
       refresh();
       // ======================= gradient + exact Hessian at x ===========================
       float H[HN];
@@ -842,7 +913,7 @@ struct Solver {
           const float hp = quad ? d * inv_beta : 1.0f;
           gx = T.w * hp * ux; gy = T.w * hp * uy; gz = T.w * hp * uz;
           const float s_iso = T.w * (quad ? inv_beta : invd);
-          const float s_rad = (quad || !exact) ? 0.f : T.w * invd;
+          const float s_rad = (quad || !bk.exact()) ? 0.f : T.w * invd;
           const float uj = s_rad * fmaf(ux, j0, fmaf(uy, j1, uz * j2));
           y0 = fmaf(s_iso, j0, -uj * ux); y1 = fmaf(s_iso, j1, -uj * uy); y2 = fmaf(s_iso, j2, -uj * uz);
         }
@@ -983,9 +1054,9 @@ struct Solver {
       const bool free_ = isvar && !act;
       const unsigned fmask = gballot<G>(free_, lane);
       const bool any_act = gany<G>(act, lane);
-      if (recheck && (fmask == last_fmask || ++rechecks >= 3)) done = true;
-      recheck = false;
-      last_fmask = fmask;
+      if (bk.recheck() && (fmask == bk.last_fmask() || bk.inc_rechecks() >= 3)) bk.set_done(true);
+      bk.set_recheck(false);
+      bk.set_last_fmask(fmask);
       // Frozen variables (active bounds, fixed / mimic lanes) get identity rows and columns.  The common case
       // -- every lane below dof is a free variable -- skips this pass entirely (warp-uniform branch); lanes
       // at or above dof have all-zero rows and are never pivots (the factorisation stops at dof).
@@ -1003,16 +1074,16 @@ struct Solver {
       if (!free_) g = 0.f;
       const float gn = gmax<G>(fabsf(g));
       bool revert = false;
-      if (trust_prev && !done) {
+      if (bk.trust_prev() && !bk.done()) {
         if (gn < gn_prev) {
           if (gn < kTrustDecrease * gn_prev) lam = fmaxf(lam * kLamDown, kLamMin);
-          stall = 0;
+          bk.clear_stall();
         } else {
           revert = true;
-          ++stall;
+          bk.inc_stall();
         }
       }
-      DEXR_TRACE_PRINT("  it %2d gn %.3e gn_prev %.3e trust_prev %d stall %d revert %d lam %.1e\n", iters, gn, gn_prev, (int)trust_prev, stall, (int)revert, lam);
+      DEXR_TRACE_PRINT("  it %2d gn %.3e gn_prev %.3e trust_prev %d stall %d revert %d lam %.1e\n", bk.iters(), gn, gn_prev, (int)bk.trust_prev(), bk.stall(), (int)revert, lam);
       float* hbuf = hb();
 #pragma unroll
       for (int i = 0; i < HN; ++i) hbuf[i * NP + l] = H[i];
@@ -1023,7 +1094,7 @@ struct Solver {
       float hd = free_ ? hbuf[dj * NP + l] + reg2 : 1.0f;
       float D = fabsf(hd) + 1e-6f;
       // ======================= damped Newton trials ====================================
-      bool accepted = done;
+      bool accepted = bk.done();
       float acc_step = 0.f;
       float Rn[9], pn[3], an[3];
       for (int trial = 0; trial < kMaxTrials; ++trial) {
@@ -1265,7 +1336,7 @@ struct Solver {
           }
         }
         if (!gany<32>(!accepted && !bad, lane)) {  // no pending group has a usable step: no FK needed
-          if (!accepted && !dropped) { lam *= kLamUp; ++rejects; }
+          if (!accepted && !dropped) { lam *= kLamUp; bk.inc_rejects(); }
           continue;
         }
         float xn = free_ ? fminf(fmaxf(x + y, lo), hi) : x;
@@ -1294,8 +1365,8 @@ struct Solver {
         // the damping is relaxed after a decrease that fp32 can resolve: one beyond the worst-case rounding bound, or one that
         // agrees with the quadratic model's prediction to within a half (rounding noise that large would not track it)
         const bool verified = !revert && (dF < -fnoise || (dF < 0.f && fabsf(dF + pred) <= 0.5f * pred));
-        DEXR_TRACE_PRINT("  it %2d trial %d lam %.1e exact %d step %.3e pred %.3e F %.9e Fn %.9e dF %.2e noise %.1e bad %d ok %d ver %d fmask %x\n", iters,
-                         trial, lam, (int)exact, step, pred, F, Fn, dF, fnoise, (int)bad, (int)ok, (int)verified, fmask);
+        DEXR_TRACE_PRINT("  it %2d trial %d lam %.1e exact %d step %.3e pred %.3e F %.9e Fn %.9e dF %.2e noise %.1e bad %d ok %d ver %d fmask %x\n", bk.iters(),
+                         trial, lam, (int)bk.exact(), step, pred, F, Fn, dF, fnoise, (int)bad, (int)ok, (int)verified, fmask);
         if (!accepted) {
           if (ok) {
             x_prev = x;
@@ -1312,51 +1383,50 @@ struct Solver {
             for (int i = 0; i < 3; ++i) p[i] = pn[i];
             cur ^= 1;
             // (see kStopAhead; not with active bounds, extra damping or the majoriser model in play)
-            const bool ahead = exact && !any_act && trial == 0 && !revert && lam <= prm.lambda0 &&
+            const bool ahead = bk.exact() && !any_act && trial == 0 && !revert && lam <= prm.lambda0 &&
                                step * fmaxf(step, kStopAheadRate * s_prev) < kStopAhead * prm.tol * s_prev;
             s_prev = (trial == 0 && !revert) ? step : 0.f;
-            if (iters == 0 && !revert) lam_carry = fmaxf(prm.lambda0, kCarry * lam);
+            if (bk.iters() == 0 && !revert) lam_carry = fmaxf(prm.lambda0, kCarry * lam);
             if (verified) lam = fmaxf(lam * kLamDown, kLamMin);
             if (verified && fabsf(dF + pred) <= kModelGood * pred) lam = fmaxf(lam * kLamDown, kLamMin);  // (kModelGood)
             // fnoise is a worst-case bound (every rounding error with the same sign); a decrease beyond an eighth of it is
             // already unlikely to be noise: such a step is kept whatever the next gradient says (it just does not relax
             // the damping).  Only steps whose effect on F is truly unresolved are put to the gradient test.
-            trust_prev = !verified && !revert && !(dF < -0.125f * fnoise);
-            if (verified) stall = 0;
+            bk.set_trust_prev(!verified && !revert && !(dF < -0.125f * fnoise));
+            if (verified) bk.clear_stall();
             gn_prev = gn;
             accepted = true;
             acc_step = step;
             if (revert) {  // back at the previous point: more damping, or the end when this is the second revert in a row
               lam *= kLamUp;
-              ++rejects;
-              if (stall >= 2) { done = true; status |= DEXR_STATUS_NOISEFLOOR; }
+              bk.inc_rejects();
+              if (bk.stall() >= 2) { bk.set_done(true); bk.flag(DEXR_STATUS_NOISEFLOOR); }
               revert = false;
             } else if (step < prm.tol || ahead) {
-              if (any_act) recheck = true;
-              else done = true;
+              if (any_act) bk.set_recheck(true);
+              else bk.set_done(true);
             }
           } else {
             if (!dropped)
             {
               lam *= kLamUp;
-              ++rejects;
+              bk.inc_rejects();
             }
           }
         }
         __syncwarp();
       }
-      if (!done) {
+      if (!bk.done()) {
         if (!accepted) {
-          if (exact) lam = prm.lambda0;  // retry this point with the majoriser model
-          else done = true;              // no descent direction left at fp32 resolution
+          if (bk.exact()) lam = prm.lambda0;  // retry this point with the majoriser model
+          else bk.set_done(true);             // no descent direction left at fp32 resolution
         }
-        exact = accepted && acc_step < kNearStep;
-        ++iters;
-        if (iters >= prm.max_iters && !done) { done = true; status |= DEXR_STATUS_MAXITER; }
+        bk.set_exact(accepted && acc_step < kNearStep);
+        bk.inc_iters();
+        if (bk.iters() >= prm.max_iters && !bk.done()) { bk.set_done(true); bk.flag(DEXR_STATUS_MAXITER); }
       }
     }
-    status |= (iters & 0xffff) | ((rejects > 127 ? 127 : rejects) << 16);
-    return status;
+    return bk.status();
   }
 };
 
