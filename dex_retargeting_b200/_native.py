@@ -17,6 +17,7 @@ TABLE_MAGIC = 0x31525844
 
 STATUS_MAXITER = 1 << 24
 STATUS_NONFINITE = 1 << 25
+STATUS_NOT_PD = 1 << 26
 
 _f, _i, _u = C.c_float, C.c_int32, C.c_uint32
 
@@ -76,6 +77,17 @@ class DexrEval(C.Structure):
     ]
 
 
+class DexrVjp(C.Structure):
+    """Mirror of `dexr_vjp_t`: buffers of one backpropagation through the solve (`dexr_solve_vjp`)."""
+
+    _fields_ = [
+        ("keypoints", C.c_void_p), ("ref_value", C.c_void_p), ("fixed_qpos", C.c_void_p), ("qpos", C.c_void_p),
+        ("last_qpos", C.c_void_p), ("projected", C.c_void_p), ("grad_qpos", C.c_void_p), ("grad_keypoints", C.c_void_p),
+        ("grad_ref_value", C.c_void_p), ("grad_fixed_qpos", C.c_void_p), ("grad_last_qpos", C.c_void_p),
+        ("status_out", C.c_void_p),
+    ]
+
+
 class DexrGroup(C.Structure):
     """Mirror of `dexr_group_t`: one (robot, batch) group of a mixed-robot launch."""
 
@@ -95,7 +107,7 @@ EXPORTS = [
     "dexr_sequences_sizeof", "dexr_default_params",
     "dexr_robot_create", "dexr_robot_create_from_device", "dexr_robot_device_table", "dexr_robot_destroy",
     "dexr_solve_frames", "dexr_solve_frames_multi", "dexr_solve_sequences", "dexr_solve_frames_host", "dexr_get_launch_info",
-    "dexr_preprocess_keypoints", "dexr_eval_sizeof", "dexr_eval_objective",
+    "dexr_preprocess_keypoints", "dexr_eval_sizeof", "dexr_eval_objective", "dexr_vjp_sizeof", "dexr_solve_vjp",
 ]
 
 _LIB = None
@@ -160,6 +172,13 @@ def load():
         lib.dexr_eval_objective.argtypes = [C.c_void_p, C.POINTER(DexrParams), C.POINTER(DexrEval), C.c_int64, C.c_void_p]
     elif not os.environ.get("DEXR_LIBRARY"):
         raise DexrError(f"{path} does not export dexr_eval_sizeof: rebuild it (python -m dex_retargeting_b200.build --force)")
+    if hasattr(lib, "dexr_vjp_sizeof"):
+        lib.dexr_vjp_sizeof.restype = C.c_size_t
+        if lib.dexr_vjp_sizeof() != C.sizeof(DexrVjp):
+            raise DexrError("dexr_vjp_t layout mismatch between library and binding (stale DEXR_LIBRARY?)")
+        lib.dexr_solve_vjp.argtypes = [C.c_void_p, C.POINTER(DexrParams), C.POINTER(DexrVjp), C.c_int64, C.c_void_p]
+    elif not os.environ.get("DEXR_LIBRARY"):
+        raise DexrError(f"{path} does not export dexr_vjp_sizeof: rebuild it (python -m dex_retargeting_b200.build --force)")
     # (an older A/B library named by DEXR_LIBRARY reads a prefix of the buffer structs -- fields are only ever appended -- so
     # the single-robot entry points still work with it; dexr_solve_frames_multi, whose groups embed the struct, does not)
     _LIB = lib

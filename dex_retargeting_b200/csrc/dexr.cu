@@ -283,6 +283,44 @@ __global__ void __launch_bounds__(kEvalWarps * 32, 2) dexr_eval_kernel(const Eva
 }
 
 // ------------------------------------------------------------------------------------------------
+// backpropagation through the solve: the evaluation kernel's launch shape, one frame per group of G lanes
+// ------------------------------------------------------------------------------------------------
+struct VjpArgs {
+  const dexr_table_t* table;
+  dexr_params_t prm;
+  dexr_vjp_t io;
+  long long B;
+  int in_row;  // floats per frame of the kp/ref input (63 or 3m)
+  Dims dm;
+  int scratch_off;
+};
+
+template <int G>
+__global__ void __launch_bounds__(kEvalWarps * 32, 2) dexr_vjp_kernel(const VjpArgs a) {
+  load_shared_table(*reinterpret_cast<SharedTable*>(dsmem), a.table);  // (the residual-pass schedule is not read)
+  __syncthreads();
+  constexpr int GPW = 32 / G;
+  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
+  const int lane = threadIdx.x & 31;
+  Solver<G, 0> sv;
+  sv.init(a.table, a.dm, (uint32_t)(a.scratch_off + (warp * GPW + lane / G) * VjpScratch<G>::kFloats * 4), a.prm, lane);
+  const bool by_kp = a.io.keypoints != nullptr;
+  const long long step = (long long)gridDim.x * kEvalWarps * GPW;
+  for (long long base = ((long long)blockIdx.x * kEvalWarps + warp) * GPW; base < a.B; base += step) {
+    const long long idx = base + lane / G;
+    const bool active = idx < a.B;
+    const long long f = active ? idx : base;
+    FrameInputs in;
+    in.kp = by_kp ? a.io.keypoints + f * a.in_row : nullptr;
+    in.ref = by_kp ? nullptr : a.io.ref_value + f * a.in_row;
+    in.fixed = a.dm.n_fixed > 0 ? a.io.fixed_qpos + f * a.dm.n_fixed : nullptr;
+    in.last = nullptr;
+    in.projected = nullptr;  // (vjp_frame reads the flags into its scratch)
+    vjp_frame(sv, in, a.io, a.dm, f, active);
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
 // keypoint pre-processing (single_hand_detector.py:100-103, 130-158): one thread per frame for the 3x3 frame,
 // tile staged through shared memory so that global loads / stores are coalesced 16-byte accesses
 // ------------------------------------------------------------------------------------------------
@@ -530,6 +568,7 @@ size_t dexr_params_sizeof(void) { return sizeof(dexr_params_t); }
 size_t dexr_frames_sizeof(void) { return sizeof(dexr_frames_t); }
 size_t dexr_sequences_sizeof(void) { return sizeof(dexr_sequences_t); }
 size_t dexr_eval_sizeof(void) { return sizeof(dexr_eval_t); }
+size_t dexr_vjp_sizeof(void) { return sizeof(dexr_vjp_t); }
 
 void dexr_default_params(dexr_params_t* p) {
   p->huber_delta = 0.02f;
@@ -762,10 +801,11 @@ static int check_loss_params(const dexr_params_t* p) {
 // CTAs per SM of the evaluation kernel: as many as are resident at once (registers and shared memory allow), one wave that
 // grid-strides over the batch.  DEXR_EVAL_CTAS_PER_SM (read per call) caps it for A/B runs.  The choice is measured in
 // DESIGN.md section 3 ("Objective evaluation").
-template <int G>
-static int eval_ctas_per_sm(int smem, int* out) {
+// The VJP kernel uses the same rule and cap.
+template <class K>
+static int eval_ctas_per_sm(K kern, int smem, int* out) {
   int resident = 0;
-  CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&resident, dexr_eval_kernel<G>, kEvalWarps * 32, smem));
+  CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&resident, kern, kEvalWarps * 32, smem));
   int n = std::max(1, resident);
   if (const char* e = getenv("DEXR_EVAL_CTAS_PER_SM"))
     if (atoi(e) > 0) n = std::min(n, atoi(e));
@@ -787,7 +827,7 @@ static int launch_eval(dexr_robot* r, const dexr_params_t* prm, const dexr_eval_
   constexpr int GPW = 32 / G;
   const int smem = a.scratch_off + kEvalWarps * GPW * eval_scratch_floats<G>() * 4;  // below the 48 KB default
   int per_sm = 1;
-  if (int e = eval_ctas_per_sm<G>(smem, &per_sm)) return e;
+  if (int e = eval_ctas_per_sm(dexr_eval_kernel<G>, smem, &per_sm)) return e;
   const long long ctas = (B + kEvalWarps * GPW - 1) / (kEvalWarps * GPW);
   const int grid = (int)std::min<long long>(ctas, (long long)r->num_sms * per_sm);
   dexr_eval_kernel<G><<<grid, kEvalWarps * 32, smem, stream>>>(a);
@@ -811,6 +851,53 @@ extern "C" int dexr_eval_objective(const dexr_robot_t* robot, const dexr_params_
   cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
   return eval_lanes(r->host) == 16 ? launch_eval<16>(r, params, io, num_frames, stream)
                                    : launch_eval<32>(r, params, io, num_frames, stream);
+}
+
+static int check_vjp_io(const dexr_table_t& t, const dexr_vjp_t* io, const dexr_params_t* prm) {
+  if (const char* msg = vjp_io_error(t, *io, *prm)) return fail(DEXR_E_INVALID, "%s", msg);
+  return 0;
+}
+
+template <int G>
+static int launch_vjp(dexr_robot* r, const dexr_params_t* prm, const dexr_vjp_t* io, long long B, cudaStream_t stream) {
+  const dexr_table_t& t = r->host;
+  VjpArgs a{};
+  a.table = r->table_dev;
+  a.prm = *prm;
+  a.io = *io;
+  a.B = B;
+  a.in_row = io->keypoints ? 3 * DEXR_NUM_KEYPOINTS : 3 * t.n_res;
+  a.dm = make_dims(t);
+  a.scratch_off = round_up((int)sizeof(SharedTable), 16);
+  constexpr int GPW = 32 / G;
+  const int smem = a.scratch_off + kEvalWarps * GPW * VjpScratch<G>::kFloats * 4;  // 16 lanes: 77 KB, 32 lanes: 101 KB
+  auto kern = dexr_vjp_kernel<G>;
+  CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  int per_sm = 1;
+  if (int e = eval_ctas_per_sm(kern, smem, &per_sm)) return e;
+  const long long ctas = (B + kEvalWarps * GPW - 1) / (kEvalWarps * GPW);
+  const int grid = (int)std::min<long long>(ctas, (long long)r->num_sms * per_sm);
+  kern<<<grid, kEvalWarps * 32, smem, stream>>>(a);
+  CUDA_TRY(cudaGetLastError());
+  {
+    std::lock_guard<std::mutex> lk(r->info_mu);
+    r->last = dexr_launch_info_t{grid, kEvalWarps * 32, smem, 0, G, kEvalWarps, r->last.kernels_launched + 1};
+  }
+  return 0;
+}
+
+extern "C" int dexr_solve_vjp(const dexr_robot_t* robot, const dexr_params_t* params, const dexr_vjp_t* io,
+                              int64_t num_frames, void* cuda_stream) {
+  if (!robot || !params || !io) return fail(DEXR_E_INVALID, "dexr_solve_vjp: null argument");
+  if (num_frames < 0) return fail(DEXR_E_INVALID, "num_frames < 0");
+  if (int e = check_vjp_io(robot->host, io, params)) return e;
+  if (int e = check_loss_params(params)) return e;
+  if (num_frames == 0) return 0;
+  DEVICE_SCOPE(robot->device);
+  dexr_robot* r = const_cast<dexr_robot*>(robot);
+  cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
+  return eval_lanes(r->host) == 16 ? launch_vjp<16>(r, params, io, num_frames, stream)
+                                   : launch_vjp<32>(r, params, io, num_frames, stream);
 }
 
 extern "C" int dexr_solve_frames_multi(const dexr_group_t* groups, int32_t num_groups, void* cuda_stream) {

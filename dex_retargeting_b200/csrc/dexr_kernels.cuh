@@ -1689,4 +1689,339 @@ __device__ __forceinline__ void evaluate_frame(Solver<G, 0>& sv, const FrameInpu
   __syncwarp();  // the group's next frame rewrites the targets and link positions this one read
 }
 
+// ------------------------------------------------------------------------------------------------
+// backpropagation through the solve (dexr_solve_vjp): implicit-function cotangents at a given point
+// ------------------------------------------------------------------------------------------------
+// At a stationary point x of F(x; theta) = L(x; theta) + norm_delta |x - a|^2 on its free variables, g(x*(theta); theta) = 0
+// gives dx*/dtheta = -H_ff^-1 dg_f/dtheta, so for a cotangent gbar = dl/dx: v_f = H_ff^-1 gbar_f, v_A = 0 on the active
+// variables, and theta_bar = -(dg/dtheta)^T v.  H is the EXACT Hessian of F -- not the solver's curvature models (no position
+// majoriser, no dropped radial term, no positive-definite fallback, no damping) -- so this runs on its own Hessian code
+// rather than solve()'s; sharing code with solve() would also change the solver kernels' machine code.  The Jacobian-column
+// and loss-derivative formulas are those of evaluate_frame, restated in vjp_column rather than factored out of it, so that the
+// evaluation kernels' machine code stays untouched.
+//
+// Per-group scratch (floats), the dense Scratch<G> layout up to kLcol followed by three small arrays:
+//   kFr, kLp   targets and link positions, as in a solve (one link buffer used)
+//   kU         jbuf[2][3][NP]: the lanes' Jacobian columns of the residual in flight; at_a / at_t: axis and torque sums of
+//              the kinematic curvature
+//   kH         [NP][NP] H_q, the joint-space Hessian of L (loss + kinematic curvature), column per lane (symmetric)
+//   kA         [NP][NP+1] M^T H_q M + 2 norm_delta I over the free variables, identity rows and columns elsewhere; row per
+//              lane, factorised in place (lower Cholesky factor)
+//   kMv        [NP] M v: the solution mapped to joint space (mimic lanes get mult * v of their source, fixed lanes 0)
+//   kKp        [64] the keypoint cotangent accumulator
+//   kFlags     16 bytes: the frame's DexPilot flags.  prepare_targets writes back the flags it reads; it gets this private
+//              copy, so the caller's `projected` is never written
+// 16 lanes: 1060 floats (4.1 KB) per group; 32 lanes: 2884 floats (11.3 KB).
+template <int G>
+struct VjpScratch {
+  static constexpr int NP = G;
+  static constexpr int kH = Scratch<G>::kHb;
+  static constexpr int kA = Scratch<G>::kLcol;
+  static constexpr int kMv = kA + NP * (NP + 1);
+  static constexpr int kKp = kMv + NP;
+  static constexpr int kFlags = kKp + 64;
+  static constexpr int kFloats = ((kFlags + 4 + 3) / 4) * 4;
+};
+static_assert(VjpScratch<16>::kFloats == 1060 && VjpScratch<32>::kFloats == 2884, "VJP scratch layout (DESIGN.md 3.8)");
+
+// The argument checks of dexr_solve_vjp that read the robot's table: nullptr, or what is wrong.  Host code shared by the
+// library and the host emulation, as eval_io_error.
+inline const char* vjp_io_error(const dexr_table_t& t, const dexr_vjp_t& io, const dexr_params_t& prm) {
+  if (!io.qpos) return "qpos is required";
+  if (!io.grad_qpos) return "grad_qpos is required";
+  if ((io.keypoints != nullptr) == (io.ref_value != nullptr)) return "exactly one of keypoints / ref_value must be given";
+  if (prm.preprocess != 0) return "raw-landmark pre-processing is not differentiated: params.preprocess must be 0";
+  if (t.n_fixed > 0 && !io.fixed_qpos) return "the robot has fixed joints but fixed_qpos is NULL";
+  if (io.grad_keypoints && !io.keypoints) return "grad_keypoints needs the keypoints form";
+  if (io.grad_ref_value && !io.ref_value) return "grad_ref_value needs the ref_value form";
+  if (io.grad_last_qpos && !io.last_qpos) return "grad_last_qpos needs last_qpos";
+  return nullptr;
+}
+
+// This lane's Jacobian column of residual k (task minus origin link) and the residual r = p_task - p_origin - target.
+template <int G>
+__device__ __forceinline__ void vjp_column(const Solver<G, 0>& sv, int k, float& j0, float& j1, float& j2, float& rx,
+                                           float& ry, float& rz) {
+  const SharedTable& st = Solver<G, 0>::ST();
+  const int l = sv.l;
+  const bool rev = sv.jtype == 0;
+  const int ti = st.res_task[k], oi = st.res_origin[k];
+  const float4 T = sv.fr()[k];
+  const float4 pt = sv.lp(0)[ti];
+  rx = pt.x - T.x; ry = pt.y - T.y; rz = pt.z - T.z;
+  j0 = 0.f; j1 = 0.f; j2 = 0.f;
+  if ((st.link_anc[ti] >> l) & 1u) {
+    if (rev) {
+      const float dx = pt.x - sv.p[0], dy = pt.y - sv.p[1], dz = pt.z - sv.p[2];
+      j0 = sv.a[1] * dz - sv.a[2] * dy; j1 = sv.a[2] * dx - sv.a[0] * dz; j2 = sv.a[0] * dy - sv.a[1] * dx;
+    } else { j0 = sv.a[0]; j1 = sv.a[1]; j2 = sv.a[2]; }
+  }
+  if (oi >= 0) {
+    const float4 po = sv.lp(0)[oi];
+    rx -= po.x; ry -= po.y; rz -= po.z;
+    if ((st.link_anc[oi] >> l) & 1u) {
+      if (rev) {
+        const float dx = po.x - sv.p[0], dy = po.y - sv.p[1], dz = po.z - sv.p[2];
+        j0 -= sv.a[1] * dz - sv.a[2] * dy; j1 -= sv.a[2] * dx - sv.a[0] * dz; j2 -= sv.a[0] * dy - sv.a[1] * dx;
+      } else { j0 -= sv.a[0]; j1 -= sv.a[1]; j2 -= sv.a[2]; }
+    }
+  }
+}
+
+// One frame of dexr_solve_vjp (see dexr.h): reads qpos, grad_qpos and the frame's inputs, writes the requested cotangents
+// and the status.  `dm` is the kernel argument's, as in evaluate_frame.
+template <int G>
+__device__ __forceinline__ void vjp_frame(Solver<G, 0>& sv, const FrameInputs& in_, const dexr_vjp_t& io, const Dims& dm,
+                                          long long f, bool active) {
+  using VS = VjpScratch<G>;
+  constexpr int NP = G;
+  const SharedTable& st = Solver<G, 0>::ST();
+  const int l = sv.l, lane = sv.lane, dof = dm.dof, m = dm.n_res;
+  const bool isvar = sv.var >= 0;
+  float* const hq = sv.scf() + VS::kH;
+  float* const A = sv.scf() + VS::kA;
+  float* const mvs = sv.scf() + VS::kMv;
+  float* const kpacc = sv.scf() + VS::kKp;
+  uint8_t* const flags = reinterpret_cast<uint8_t*>(sv.scf() + VS::kFlags);
+
+  // ---- inputs, targets (flags on the private copy), FK at x
+  float x = 0.f, x0 = 0.f, gbar = 0.f;
+  if (active && isvar) {
+    x = io.qpos[f * dm.n_var + sv.var];
+    x0 = io.last_qpos ? io.last_qpos[f * dm.n_var + sv.var] : x;
+    gbar = io.grad_qpos[f * dm.n_var + sv.var];
+  }
+  const int fixedi = st.fixed_index[l];
+  sv.qfix = (active && fixedi >= 0) ? in_.fixed[fixedi] : 0.f;
+  sv.x = x;
+  if (l < dm.len_proj) flags[l] = (active && io.projected) ? io.projected[f * dm.len_proj + l] : (uint8_t)0;
+  for (int e = l; e < 64; e += G) kpacc[e] = 0.f;
+  __syncwarp();
+  FrameInputs in = in_;
+  in.projected = dm.len_proj > 0 ? flags : nullptr;
+  bool finite = isfinite(x) && isfinite(x0) && isfinite(sv.qfix) && isfinite(gbar);
+  const bool ok_targets = sv.prepare_targets(in, active);
+  finite = !gany<G>(!finite, lane) && ok_targets;
+  __syncwarp();
+  sv.q = sv.compose_q(x);
+  {
+    float R[9];
+    sv.fk(sv.q, R, sv.p);
+    sv.write_world_links();
+    sv.write_links(R, sv.p, 0);
+    sv.set_world_axis(R);
+  }
+  __syncwarp();
+
+  // ---- gradient of F and H_q, one residual per pass: loss curvature J^T (d2h/dr2) J, then the kinematic curvature
+  const float nd = io.last_qpos ? sv.prm.norm_delta : 0.f;  // no anchor: no regulariser
+  const float beta = sv.prm.huber_delta, inv_beta = sv.inv_beta;
+  const bool pos_loss = dm.loss == DEXR_LOSS_POSITION;
+  float H[NP];
+#pragma unroll
+  for (int i = 0; i < NP; ++i) H[i] = 0.f;
+  float g = 0.f, t0 = 0.f, t1 = 0.f, t2 = 0.f;
+  for (int k = 0; k < m; ++k) {
+    float j0, j1, j2, rx, ry, rz;
+    vjp_column(sv, k, j0, j1, j2, rx, ry, rz);
+    const float w = sv.fr()[k].w;
+    float gx, gy, gz, y0, y1, y2;  // dh/dr and (d2h/dr2) j
+    if (pos_loss) {
+      // per-coordinate Huber: curvature w / beta inside the quadratic zone, exactly 0 beyond it
+      const float ax_ = fabsf(rx), ay_ = fabsf(ry), az_ = fabsf(rz);
+      gx = w * rx * (ax_ < beta ? inv_beta : fast_rcp(ax_));
+      gy = w * ry * (ay_ < beta ? inv_beta : fast_rcp(ay_));
+      gz = w * rz * (az_ < beta ? inv_beta : fast_rcp(az_));
+      y0 = ax_ < beta ? w * inv_beta * j0 : 0.f;
+      y1 = ay_ < beta ? w * inv_beta * j1 : 0.f;
+      y2 = az_ < beta ? w * inv_beta * j2 : 0.f;
+    } else {
+      // Huber of the norm: w I / beta for d < beta, w (I - u u^T) / d beyond (the radial curvature is exactly 0 there)
+      const float d = sqrtf(fmaf(rx, rx, fmaf(ry, ry, rz * rz)));
+      const bool quad = d < beta;
+      const float invd = d > 1e-30f ? fast_rcp(d) : 0.f;
+      const float ux = rx * invd, uy = ry * invd, uz = rz * invd;
+      const float hp = quad ? d * inv_beta : 1.0f;
+      gx = w * hp * ux; gy = w * hp * uy; gz = w * hp * uz;
+      const float s_iso = w * (quad ? inv_beta : invd);
+      const float uj = (quad ? 0.f : w * invd) * fmaf(ux, j0, fmaf(uy, j1, uz * j2));
+      y0 = fmaf(s_iso, j0, -uj * ux); y1 = fmaf(s_iso, j1, -uj * uy); y2 = fmaf(s_iso, j2, -uj * uz);
+    }
+    g = fmaf(j0, gx, fmaf(j1, gy, fmaf(j2, gz, g)));
+    t0 += j1 * gz - j2 * gy; t1 += j2 * gx - j0 * gz; t2 += j0 * gy - j1 * gx;
+    const int b = k & 1;
+    sv.jbuf(b, 0)[l] = j0; sv.jbuf(b, 1)[l] = j1; sv.jbuf(b, 2)[l] = j2;
+    __syncwarp();
+#pragma unroll
+    for (int c4 = 0; c4 < NP; c4 += 4) {
+      const float4 c0 = *reinterpret_cast<const float4*>(sv.jbuf(b, 0) + c4);
+      const float4 c1 = *reinterpret_cast<const float4*>(sv.jbuf(b, 1) + c4);
+      const float4 c2 = *reinterpret_cast<const float4*>(sv.jbuf(b, 2) + c4);
+      H[c4 + 0] = fmaf(c0.x, y0, fmaf(c1.x, y1, fmaf(c2.x, y2, H[c4 + 0])));
+      H[c4 + 1] = fmaf(c0.y, y0, fmaf(c1.y, y1, fmaf(c2.y, y2, H[c4 + 1])));
+      H[c4 + 2] = fmaf(c0.z, y0, fmaf(c1.z, y1, fmaf(c2.z, y2, H[c4 + 2])));
+      H[c4 + 3] = fmaf(c0.w, y0, fmaf(c1.w, y1, fmaf(c2.w, y2, H[c4 + 3])));
+    }
+  }
+  {
+    // kinematic curvature (as in solve()): S[l][i] = a_i . t_l for i ancestor-or-self of l, a_l . t_i for i below l, with
+    // t_c = sum_k J_kc x dh/dr_k and a the world axis of a revolute joint (0 for a prismatic one)
+    const bool rev = sv.jtype == 0;
+    const float ar0 = rev ? sv.a[0] : 0.f, ar1 = rev ? sv.a[1] : 0.f, ar2 = rev ? sv.a[2] : 0.f;
+    sv.at_a(l) = make_float4(ar0, ar1, ar2, 0.f);
+    sv.at_t(l) = make_float4(t0, t1, t2, 0.f);
+    __syncwarp();
+#pragma unroll
+    for (int i = 0; i < NP; ++i) {
+      if (i < dof) {
+        const float4 ai = sv.at_a(i), ti_ = sv.at_t(i);
+        const bool up = (sv.anc >> i) & 1u, dn = (sv.desc >> i) & 1u;
+        const float vu = fmaf(ai.x, t0, fmaf(ai.y, t1, ai.z * t2));
+        const float vd = fmaf(ar0, ti_.x, fmaf(ar1, ti_.y, ar2 * ti_.z));
+        H[i] += up ? vu : (dn ? vd : 0.f);
+      }
+    }
+  }
+#pragma unroll
+  for (int i = 0; i < NP; ++i) hq[i * NP + l] = H[i];
+  // g_x = M^T g_q + 2 norm_delta (x - a), as in evaluate_frame
+  if (dm.has_mimic) {
+    const int gcount = st.group_count[l];
+    float gx_ = 0.f;
+#pragma unroll
+    for (int k = 0; k < DEXR_MAX_GROUP; ++k) {
+      const bool v = isvar && k < gcount;
+      const float gv = gshfl<G>(g, v ? st.group_lane[l][k] : l);
+      if (v) gx_ = fmaf(st.group_mult[l][k], gv, gx_);
+    }
+    g = gx_;
+  }
+  g = isvar ? fmaf(2.0f * nd, x - x0, g) : 0.f;
+
+  // ---- active set (the solver's rule at its widened bounds), then A = the free block of M^T H_q M + 2 norm_delta I
+  const bool act = isvar && ((x <= sv.lo && g > -kGradNoise) || (x >= sv.hi && g < kGradNoise));
+  const bool free_ = isvar && !act;
+  const unsigned fmask = gballot<G>(free_, lane);
+  __syncwarp();
+  {
+    const int gca = free_ ? st.group_count[l] : 0;
+    for (int c = 0; c < dof; ++c) {
+      float h = c == l ? 1.0f : 0.f;
+      if (free_ && ((fmask >> c) & 1u)) {
+        h = c == l ? 2.0f * nd : 0.f;
+        const int gcb = st.group_count[c];
+        for (int fb = 0; fb < gcb; ++fb) {
+          const float* col = hq + st.group_lane[c][fb] * NP;
+          const float mb = st.group_mult[c][fb];
+          for (int fa = 0; fa < gca; ++fa) h = fmaf(mb * st.group_mult[l][fa], col[st.group_lane[l][fa]], h);
+        }
+      }
+      A[l * (NP + 1) + c] = h;
+    }
+  }
+  // ---- Cholesky of A in place, lane = row, one pivot column per step (fp32, IEEE sqrt and division)
+  bool bad = false;
+  for (int k = 0; k < dof; ++k) {
+    __syncwarp();
+    const float d = A[k * (NP + 1) + k];
+    bad = bad || !(d > 0.f);  // a pivot <= 0: not a strict local minimum of the free subproblem
+    const float lkk = sqrtf(fmaxf(d, 1e-30f));
+    __syncwarp();
+    if (l == k) A[k * (NP + 1) + k] = lkk;
+    else if (l > k && l < dof) A[l * (NP + 1) + k] /= lkk;
+    __syncwarp();
+    if (l > k && l < dof) {
+      const float lik = A[l * (NP + 1) + k];
+      for (int j = k + 1; j <= l; ++j) A[l * (NP + 1) + j] = fmaf(-lik, A[j * (NP + 1) + k], A[l * (NP + 1) + j]);
+    }
+  }
+  __syncwarp();
+  // v = A^-1 gbar (forward, then back substitution; frozen rows are identity rows with a zero right-hand side)
+  float y = free_ ? gbar : 0.f;
+  for (int k = 0; k < dof; ++k) {
+    const float yk = gshfl<G>(y, k) / A[k * (NP + 1) + k];
+    if (l == k) y = yk;
+    else if (l > k && l < dof) y = fmaf(-A[l * (NP + 1) + k], yk, y);
+  }
+  for (int k = dof - 1; k >= 0; --k) {
+    const float vk = gshfl<G>(y, k) / A[k * (NP + 1) + k];
+    if (l == k) y = vk;
+    else if (l < k) y = fmaf(-A[k * (NP + 1) + l], vk, y);
+  }
+  const float v = bad ? 0.f : y;
+  {
+    const float vsrc = gshfl<G>(v, sv.msrc >= 0 ? sv.msrc : l);
+    mvs[l] = isvar ? v : (sv.msrc >= 0 ? sv.mmult * vsrc : 0.f);
+  }
+  __syncwarp();
+  const float mv = mvs[l];
+  // outputs: NaN for a frame with a non-finite input, 0 for one whose free Hessian is not positive definite
+  auto out = [&](float val) { return !finite ? __int_as_float(0x7fc00000) : (bad ? 0.f : val); };
+
+  // ---- targets: t_bar_k = (d2h/dr2)(r_k) J_k M v, then through the target map back to ref_value / keypoints
+  const bool by_kp = in.kp != nullptr;
+  for (int k = 0; k < m; ++k) {
+    float j0, j1, j2, rx, ry, rz;
+    vjp_column(sv, k, j0, j1, j2, rx, ry, rz);
+    const float u0 = gsum<G>(j0 * mv), u1 = gsum<G>(j1 * mv), u2 = gsum<G>(j2 * mv);  // J_k M v
+    const float w = sv.fr()[k].w;
+    float b0, b1, b2;
+    if (pos_loss) {
+      b0 = fabsf(rx) < beta ? w * inv_beta * u0 : 0.f;
+      b1 = fabsf(ry) < beta ? w * inv_beta * u1 : 0.f;
+      b2 = fabsf(rz) < beta ? w * inv_beta * u2 : 0.f;
+    } else {
+      const float d = sqrtf(fmaf(rx, rx, fmaf(ry, ry, rz * rz)));
+      const bool quad = d < beta;
+      const float invd = d > 1e-30f ? fast_rcp(d) : 0.f;
+      const float ux = rx * invd, uy = ry * invd, uz = rz * invd;
+      const float s_iso = w * (quad ? inv_beta : invd);
+      const float uu = (quad ? 0.f : w * invd) * fmaf(ux, u0, fmaf(uy, u1, uz * u2));
+      b0 = fmaf(s_iso, u0, -uu * ux); b1 = fmaf(s_iso, u1, -uu * uy); b2 = fmaf(s_iso, u2, -uu * uz);
+    }
+    const int ht = st.res_ht[k], ho = st.res_ho[k];
+    float c0 = b0, c1 = b1, c2 = b2;
+    if (!pos_loss) {
+      if (dm.loss == DEXR_LOSS_DEXPILOT && k < dm.len_proj && flags[k]) {
+        // projected pair t = eta e / (|e| + 1e-6), e the human vector: dt/de = eta / (|e| + eps) (I - e e^T / (|e| (|e| + eps)))
+        float ex, ey, ez;
+        if (by_kp) {
+          ex = in.kp[3 * ht] - in.kp[3 * ho]; ey = in.kp[3 * ht + 1] - in.kp[3 * ho + 1]; ez = in.kp[3 * ht + 2] - in.kp[3 * ho + 2];
+        } else {
+          ex = in.ref[3 * k]; ey = in.ref[3 * k + 1]; ez = in.ref[3 * k + 2];
+        }
+        const float dist = sqrtf(fmaf(ex, ex, fmaf(ey, ey, ez * ez)));
+        const float den = dist + 1e-6f;
+        const float sc = (k < dm.len_s1 ? sv.prm.eta1 : sv.prm.eta2) / den;
+        const float de = dist > 0.f ? fmaf(ex, b0, fmaf(ey, b1, ez * b2)) / (dist * den) : 0.f;
+        c0 = sc * fmaf(-de, ex, b0); c1 = sc * fmaf(-de, ey, b1); c2 = sc * fmaf(-de, ez, b2);
+      } else {
+        c0 = sv.prm.scaling * b0; c1 = sv.prm.scaling * b1; c2 = sv.prm.scaling * b2;
+      }
+    }
+    const float cl = l == 0 ? c0 : (l == 1 ? c1 : c2);
+    if (by_kp) {
+      if (l < 3) {  // keypoints shared by several residuals (the wrist) accumulate; lane c owns coordinate c
+        kpacc[3 * ht + l] += cl;
+        if (ho >= 0) kpacc[3 * ho + l] -= cl;
+      }
+    } else if (active && io.grad_ref_value && l < 3) {
+      io.grad_ref_value[(f * m + k) * 3 + l] = out(cl);
+    }
+  }
+  // ---- fixed joints: q_bar_c = -H_q[c, :] . M v; anchor: a_bar = 2 norm_delta v
+  float qbar = 0.f;
+  if (fixedi >= 0)
+    for (int i = 0; i < dof; ++i) qbar = fmaf(hq[i * NP + l], mvs[i], qbar);
+  __syncwarp();
+  if (active) {
+    if (isvar && io.grad_last_qpos) io.grad_last_qpos[f * dm.n_var + sv.var] = out(2.0f * nd * v);
+    if (fixedi >= 0 && io.grad_fixed_qpos) io.grad_fixed_qpos[f * dm.n_fixed + fixedi] = out(-qbar);
+    if (by_kp && io.grad_keypoints)
+      for (int e = l; e < 3 * DEXR_NUM_KEYPOINTS; e += G) io.grad_keypoints[f * 3 * DEXR_NUM_KEYPOINTS + e] = out(kpacc[e]);
+    if (l == 0 && io.status_out) io.status_out[f] = !finite ? DEXR_STATUS_NONFINITE : (bad ? DEXR_STATUS_NOT_PD : 0);
+  }
+  __syncwarp();  // the group's next frame rewrites the scratch this one read
+}
+
 }  // namespace dexr

@@ -5,6 +5,10 @@ objective a solve minimises, used as a training loss).
 `qpos` [B,opt_dof] (`Optimizer.objective_batch`, one `dexr_eval_objective` launch); backward returns
 grad_output[:, None] * d cost / d qpos from the same launch.  Derivatives with respect to the keypoints, the fixed joints
 or the anchor are not computed: those arguments must not require grad.
+
+`differentiable_retarget(opt, ...)` is the other direction: the solve's answer as a differentiable function of the keypoints
+(or ref_value), the fixed joints and the anchor (`Optimizer.retarget_batch` forward, `Optimizer.retarget_batch_vjp` backward):
+a hand-pose network trained with a loss on the robot joint angles backpropagates through the retargeting with it.
 """
 from __future__ import annotations
 
@@ -36,3 +40,53 @@ def retargeting_cost(opt, qpos, *, keypoints=None, ref_value=None, fixed_qpos=No
     kwargs = dict(keypoints=keypoints, ref_value=ref_value, fixed_qpos=fixed_qpos, last_qpos=last_qpos, projected=projected,
                   raw_hand=raw_hand)
     return _RetargetingCost.apply(qpos, opt, kwargs)
+
+
+class _DifferentiableRetarget(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, targets, fixed_qpos, last_qpos, opt, cfg):
+        by_kp, projected, clip_init = cfg["by_kp"], cfg["projected"], cfg["clip_init"]
+        tgt = dict(keypoints=targets) if by_kp else dict(ref_value=targets)
+        if projected is None and opt.retargeting_type == "DEXPILOT":
+            # the backward needs the flags the solve leaves; every frame starts unprojected, as with no flag buffer
+            projected = torch.zeros((targets.shape[0], opt._objective_spec().len_proj), dtype=torch.uint8,
+                                    device=targets.device)
+        kw = {k: v.detach() for k, v in tgt.items()}
+        if cfg["raw_hand"] is not None:
+            kw["raw_hand"] = cfg["raw_hand"]
+        qpos = opt.retarget_batch(fixed_qpos=None if fixed_qpos is None else fixed_qpos.detach(), last_qpos=last_qpos.detach(),
+                                  projected=projected, clip_init=clip_init, **kw)
+        flags = None if projected is None else projected.clone()
+        ctx.opt, ctx.by_kp = opt, by_kp
+        ctx.save_for_backward(qpos, targets.detach(), None if fixed_qpos is None else fixed_qpos.detach(), last_qpos.detach(),
+                              flags)
+        return qpos
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_qpos):
+        qpos, targets, fixed_qpos, last_qpos, flags = ctx.saved_tensors
+        tgt = dict(keypoints=targets) if ctx.by_kp else dict(ref_value=targets)
+        g_tgt, g_fixed, g_last = ctx.opt.retarget_batch_vjp(grad_qpos.contiguous(), qpos, fixed_qpos=fixed_qpos,
+                                                            last_qpos=last_qpos, projected=flags, **tgt)
+        return g_tgt, g_fixed, g_last, None, None
+
+
+def differentiable_retarget(opt, *, keypoints=None, ref_value=None, fixed_qpos=None, last_qpos, projected=None,
+                            clip_init=False, raw_hand=None):
+    """qpos [B,opt_dof] = `opt.retarget_batch(...)` (float32 CUDA tensors as there), differentiable in `keypoints` or
+    `ref_value`, in `fixed_qpos` and in `last_qpos` as the anchor of the norm_delta term (its warm-start role only picks the
+    basin).  backward() is one `Optimizer.retarget_batch_vjp` launch: the implicit-function derivative of the converged
+    solution (active bounds get zero sensitivity; a frame that ended at max_iters gets the derivative of the linearisation at
+    its answer; one whose free Hessian is not positive definite gets zero gradients).  `projected` (DexPilot flags) is updated
+    in place by the solve, as by `retarget_batch`; the backward uses a copy of the flags the solve left.
+    Chaining calls with one frame's output as the next call's `last_qpos` backpropagates through a stream fed frame by
+    frame.  Raw detector landmarks (`raw_hand`) are solved but not differentiated: pre-process them first."""
+    if (keypoints is None) == (ref_value is None):
+        raise ValueError("give exactly one of keypoints / ref_value")
+    targets = keypoints if keypoints is not None else ref_value
+    if raw_hand is not None and any(t is not None and t.requires_grad for t in (targets, fixed_qpos, last_qpos)):
+        raise ValueError("raw_hand: raw-landmark pre-processing is not differentiated; pre-process the keypoints "
+                         "(dexr_preprocess_keypoints) and pass them without raw_hand")
+    cfg = dict(by_kp=keypoints is not None, projected=projected, clip_init=clip_init, raw_hand=raw_hand)
+    return _DifferentiableRetarget.apply(targets, fixed_qpos, last_qpos, opt, cfg)

@@ -440,6 +440,53 @@ class Optimizer:
                 "dexr_eval_objective")
         return loss_out, cost_out, grad_out
 
+    # ---------------------------------------------------------------- backpropagation through the solve
+    def retarget_batch_vjp(self, grad_qpos, qpos, ref_value=None, fixed_qpos=None, last_qpos=None, *, keypoints=None,
+                           projected=None, grad_keypoints_out=None, grad_ref_value_out=None, grad_fixed_qpos_out=None,
+                           grad_last_qpos_out=None, status_out=None, stream=None):
+        """Backpropagate B cotangents `grad_qpos` = dl/dqpos [B,opt_dof] through the solve, one launch (`dexr_solve_vjp`).
+        `qpos` [B,opt_dof] is the solve's answer for the same inputs (tensors as for `retarget_batch`); `last_qpos` is the
+        anchor of the norm_delta term (None: no regulariser); `projected` [B,len_proj] uint8 are the DexPilot flags the solve
+        left, read only.  The derivative is the implicit-function one at a stationary point: active bounds get zero
+        sensitivity, the free variables H_ff^-1 of the exact Hessian (see include/dexr.h).
+        Returns (grad_targets, grad_fixed_qpos, grad_last_qpos), CUDA tensors: grad_targets in the form that was given
+        ([B,21,3] for keypoints, [B,m,3] for ref_value), grad_fixed_qpos None without fixed joints, grad_last_qpos None
+        without last_qpos.  `status_out` [B] int32 receives 0, STATUS_NONFINITE (non-finite outputs) or STATUS_NOT_PD (the
+        free Hessian is not positive definite: zero outputs).  Nothing is synchronised."""
+        import torch
+
+        eng = self.engine()
+        dev = torch.device("cuda", eng.device)
+        chk = _tensor_check(dev)
+        B = qpos.shape[0]
+        n, nf = self.opt_dof, len(self.idx_pin2fixed)
+        io = N.DexrVjp()
+        io.qpos = chk(qpos, (B, n), torch.float32, "qpos")
+        io.grad_qpos = chk(grad_qpos, (B, n), torch.float32, "grad_qpos")
+        self._batch_targets(io, chk, B, ref_value, keypoints, fixed_qpos, last_qpos=last_qpos)
+        if projected is not None:
+            io.projected = chk(projected, (B, self._objective_spec().len_proj), torch.uint8, "projected")
+
+        def out(t, shape, name):
+            t = torch.empty(shape, dtype=torch.float32, device=dev) if t is None else t
+            return t, chk(t, shape, torch.float32, name)
+
+        if keypoints is not None:
+            g_tgt, io.grad_keypoints = out(grad_keypoints_out, (B, N.NUM_KEYPOINTS, 3), "grad_keypoints_out")
+        else:
+            g_tgt, io.grad_ref_value = out(grad_ref_value_out, (B, self.num_residuals, 3), "grad_ref_value_out")
+        g_fixed = g_last = None
+        if nf:
+            g_fixed, io.grad_fixed_qpos = out(grad_fixed_qpos_out, (B, nf), "grad_fixed_qpos_out")
+        if last_qpos is not None:
+            g_last, io.grad_last_qpos = out(grad_last_qpos_out, (B, n), "grad_last_qpos_out")
+        if status_out is not None:
+            io.status_out = chk(status_out, (B,), torch.int32, "status_out")
+        p = self.params()
+        s = stream if stream is not None else torch.cuda.current_stream(dev)
+        N.check(eng.lib.dexr_solve_vjp(eng.handle, C.byref(p), C.byref(io), B, C.c_void_p(s.cuda_stream)), "dexr_solve_vjp")
+        return g_tgt, g_fixed, g_last
+
     def _objective_flags(self):
         """Hysteresis state an objective closure starts from (DexPilot only)."""
         return None

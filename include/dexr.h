@@ -284,6 +284,39 @@ size_t dexr_eval_sizeof(void);
 int dexr_eval_objective(const dexr_robot_t* robot, const dexr_params_t* params, const dexr_eval_t* io,
                         int64_t num_frames, void* cuda_stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Backpropagation through the solve (vector-Jacobian product of the implicit function theorem).  At a point x of frame f
+ * (normally what dexr_solve_frames returned for the same inputs) and a cotangent dl/dx, writes dl/dtheta for the frame's
+ * inputs theta: the keypoints or ref_value, the fixed joints and the anchor last_qpos.  x is taken as a stationary point of
+ * F(x) = L(x) + norm_delta |x - last_qpos|^2 on its free variables: a variable at a (widened) bound whose gradient does not
+ * point inward is active and gets zero sensitivity; for the free ones v = H_ff^-1 dl/dx_f with H the exact Hessian of F
+ * (exact Huber curvature, kinematic curvature, mimic fold), and every input cotangent is -(dg/dtheta)^T v.  A frame that
+ * ended at max_iters gets the derivative of this linearisation at the point given.  Targets are prepared as by the solve:
+ * DexPilot flags are read from `projected` (normally the flags the solve left) and never written; flags and Huber zones are
+ * piecewise constant, so the derivative is the one-sided one at a switch.  params.preprocess must be 0 (raw landmarks are not
+ * differentiated).  Asynchronous on `cuda_stream`, allocates nothing; num_frames == 0 does nothing.  A frame with a
+ * non-finite input gets non-finite outputs and DEXR_STATUS_NONFINITE; a frame whose free Hessian is not positive definite
+ * (not a strict local minimum) gets zero cotangents and DEXR_STATUS_NOT_PD.  All pointers are DEVICE pointers.
+ * ------------------------------------------------------------------------------------------- */
+#define DEXR_STATUS_NOT_PD (1 << 26)
+typedef struct dexr_vjp {
+  const float* keypoints;   /* [B,21,3] or NULL  } exactly one of the two                                            */
+  const float* ref_value;   /* [B,m,3]  or NULL  }                                                                   */
+  const float* fixed_qpos;  /* [B,n_fixed] or NULL when n_fixed == 0                                                 */
+  const float* qpos;        /* [B,n_var] the point x                                                                 */
+  const float* last_qpos;   /* [B,n_var] the anchor of the norm_delta term, or NULL: no regulariser                  */
+  const uint8_t* projected; /* [B,len_proj] DexPilot flags, read only; NULL: every flag as prepare_targets sets it from 0 */
+  const float* grad_qpos;   /* [B,n_var] dl/dx                                                                       */
+  float* grad_keypoints;    /* [B,21,3] or NULL: dl/dkeypoints (keypoints form only; all 63 entries written)         */
+  float* grad_ref_value;    /* [B,m,3]  or NULL: dl/dref_value (ref_value form only)                                 */
+  float* grad_fixed_qpos;   /* [B,n_fixed] or NULL                                                                   */
+  float* grad_last_qpos;    /* [B,n_var] or NULL: dl/dlast_qpos (needs last_qpos)                                    */
+  int32_t* status_out;      /* [B] or NULL: 0, DEXR_STATUS_NONFINITE or DEXR_STATUS_NOT_PD                           */
+} dexr_vjp_t;
+size_t dexr_vjp_sizeof(void);
+int dexr_solve_vjp(const dexr_robot_t* robot, const dexr_params_t* params, const dexr_vjp_t* io, int64_t num_frames,
+                   void* cuda_stream);
+
 #ifdef __cplusplus
 }
 #endif
