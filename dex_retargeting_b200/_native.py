@@ -88,6 +88,24 @@ class DexrVjp(C.Structure):
     ]
 
 
+class DexrSequencesTape(C.Structure):
+    """Mirror of `dexr_sequences_tape_t`: what `dexr_solve_sequences_tape` records for the backward."""
+
+    _fields_ = [("qpos", C.c_void_p), ("projected", C.c_void_p)]
+
+
+class DexrSequencesVjp(C.Structure):
+    """Mirror of `dexr_sequences_vjp_t`: buffers of one backpropagation through the sequence solve."""
+
+    _fields_ = [
+        ("keypoints", C.c_void_p), ("fixed_qpos", C.c_void_p), ("last_qpos", C.c_void_p), ("filter_init", C.c_void_p),
+        ("qpos", C.c_void_p), ("projected", C.c_void_p), ("grad_robot_qpos", C.c_void_p),
+        ("grad_last_qpos_out", C.c_void_p), ("grad_filter_state_out", C.c_void_p), ("grad_keypoints", C.c_void_p),
+        ("grad_fixed_qpos", C.c_void_p), ("grad_last_qpos", C.c_void_p), ("grad_filter_state", C.c_void_p),
+        ("status_out", C.c_void_p),
+    ]
+
+
 class DexrGroup(C.Structure):
     """Mirror of `dexr_group_t`: one (robot, batch) group of a mixed-robot launch."""
 
@@ -108,6 +126,7 @@ EXPORTS = [
     "dexr_robot_create", "dexr_robot_create_from_device", "dexr_robot_device_table", "dexr_robot_destroy",
     "dexr_solve_frames", "dexr_solve_frames_multi", "dexr_solve_sequences", "dexr_solve_frames_host", "dexr_get_launch_info",
     "dexr_preprocess_keypoints", "dexr_eval_sizeof", "dexr_eval_objective", "dexr_vjp_sizeof", "dexr_solve_vjp",
+    "dexr_sequences_tape_sizeof", "dexr_solve_sequences_tape", "dexr_sequences_vjp_sizeof", "dexr_solve_sequences_vjp",
 ]
 
 _LIB = None
@@ -179,6 +198,20 @@ def load():
         lib.dexr_solve_vjp.argtypes = [C.c_void_p, C.POINTER(DexrParams), C.POINTER(DexrVjp), C.c_int64, C.c_void_p]
     elif not os.environ.get("DEXR_LIBRARY"):
         raise DexrError(f"{path} does not export dexr_vjp_sizeof: rebuild it (python -m dex_retargeting_b200.build --force)")
+    if hasattr(lib, "dexr_sequences_vjp_sizeof"):
+        lib.dexr_sequences_tape_sizeof.restype = C.c_size_t
+        lib.dexr_sequences_vjp_sizeof.restype = C.c_size_t
+        if (lib.dexr_sequences_tape_sizeof() != C.sizeof(DexrSequencesTape)
+                or lib.dexr_sequences_vjp_sizeof() != C.sizeof(DexrSequencesVjp)):
+            raise DexrError("dexr_sequences_tape_t / dexr_sequences_vjp_t layout mismatch between library and binding "
+                            "(stale DEXR_LIBRARY?)")
+        lib.dexr_solve_sequences_tape.argtypes = [C.c_void_p, C.POINTER(DexrParams), C.POINTER(DexrSequences),
+                                                  C.POINTER(DexrSequencesTape), C.c_int64, C.c_int64, C.c_void_p]
+        lib.dexr_solve_sequences_vjp.argtypes = [C.c_void_p, C.POINTER(DexrParams), C.POINTER(DexrSequencesVjp), C.c_int64,
+                                                 C.c_int64, C.c_void_p]
+    elif not os.environ.get("DEXR_LIBRARY"):
+        raise DexrError(f"{path} does not export dexr_sequences_vjp_sizeof: rebuild it "
+                        "(python -m dex_retargeting_b200.build --force)")
     # (an older A/B library named by DEXR_LIBRARY reads a prefix of the buffer structs -- fields are only ever appended -- so
     # the single-robot entry points still work with it; dexr_solve_frames_multi, whose groups embed the struct, does not)
     _LIB = lib

@@ -239,6 +239,41 @@ __global__ void __launch_bounds__(NW * 32, 1) dexr_sequences_kernel(const SeqArg
   }
 }
 
+// dexr_solve_sequences_tape: dexr_sequences_kernel line for line, with solve_stream's recording switched on.  (A body shared
+// through an inline function changes how ptxas orders the filter test of dexr_sequences_kernel; this twin leaves that
+// kernel's machine code as it was.)
+template <int G, int BW, int NW>
+__global__ void __launch_bounds__(NW * 32, 1) dexr_sequences_tape_kernel(const SeqArgs a, const dexr_sequences_tape_t tape) {
+  unsigned char* const smem = dsmem;
+  SharedTable* st = reinterpret_cast<SharedTable*>(smem);
+  load_shared_table(*st, a.table, pass_slot_width<BW>());
+  __syncthreads();
+
+  constexpr int GPW = 32 / G;
+  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
+  const int lane = threadIdx.x & 31;
+  const int gid = warp * GPW + (lane / G);               // scratch slot of this group of lanes
+  const int slots_per_cta = NW * a.spw;
+  const uint32_t scratch_off = (uint32_t)(a.scratch_off + gid * Scratch<G, BW>::kStreamFloats * 4);
+  float* kpbuf = reinterpret_cast<float*>(smem + scratch_off) + Scratch<G, BW>::kFloats;  // 63 floats: current keypoints
+  const int slot = a.spw == GPW ? gid : warp;            // which of the CTA's stream slots this group serves
+  const bool first = (lane / G) == 0;
+  const bool owner = a.spw == GPW || first;              // the group that reads and writes the stream's state
+  const bool works = owner || a.duo;                     // (scarce streams, 16 lanes: the second half-warp helps the first)
+  Solver<G, BW> sv;
+  sv.init(a.table, a.dm, scratch_off, a.prm, lane);
+  if (G == 16 && a.duo) sv.duo = lane / G;
+  const bool use_filter = a.prm.lp_alpha >= 0.f && a.prm.lp_alpha <= 1.f;
+
+  // Streams are dealt round-robin over CTAs (stream = blockIdx + gridDim * slot): with few streams every SM gets
+  // one or two warps instead of a few SMs getting eight -- the path is latency bound per stream.
+  for (long long base = 0; base < a.S; base += (long long)gridDim.x * slots_per_cta) {
+    const long long s = base + (long long)slot * gridDim.x + blockIdx.x;
+    solve_stream<G, BW, true>(sv, a.io, a.dm, a.prm, a.S, a.steps, s, works && s < a.S, owner && s < a.S, kpbuf, use_filter,
+                              tape.qpos, tape.projected);
+  }
+}
+
 // ------------------------------------------------------------------------------------------------
 // objective evaluation: one frame per group of G lanes, groups striding over the batch
 // ------------------------------------------------------------------------------------------------
@@ -317,6 +352,45 @@ __global__ void __launch_bounds__(kEvalWarps * 32, 2) dexr_vjp_kernel(const VjpA
     in.last = nullptr;
     in.projected = nullptr;  // (vjp_frame reads the flags into its scratch)
     vjp_frame(sv, in, a.io, a.dm, f, active);
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
+// backpropagation through the sequence solve: one stream per group of G lanes, walked from its last frame to its first
+// ------------------------------------------------------------------------------------------------
+struct SeqVjpArgs {
+  const dexr_table_t* table;
+  dexr_params_t prm;
+  dexr_sequences_vjp_t io;
+  long long S;
+  int steps;
+  Dims dm;
+  int scratch_off;
+  int spw;  // streams per warp: 32 / G, or 1 (the second group of a 16-lane warp walks stream S - 1 and writes nothing)
+};
+
+// (32 lanes: a minimum of 2 CTAs per SM caps the kernel at 128 registers, and ptxas spills 4 bytes there)
+template <int G>
+__global__ void __launch_bounds__(kEvalWarps * 32, G == 16 ? 2 : 1) dexr_seq_vjp_kernel(const SeqVjpArgs a) {
+  load_shared_table(*reinterpret_cast<SharedTable*>(dsmem), a.table);  // (the residual-pass schedule is not read)
+  __syncthreads();
+  constexpr int GPW = 32 / G;
+  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
+  const int lane = threadIdx.x & 31;
+  const int gid = warp * GPW + lane / G;
+  Solver<G, 0> sv;
+  sv.init(a.table, a.dm, (uint32_t)(a.scratch_off + gid * VjpScratch<G>::kFloats * 4), a.prm, lane);
+  const int slot = a.spw == GPW ? gid : warp;
+  const bool owner = a.spw == GPW || lane < G;
+  const bool use_filter = a.prm.lp_alpha >= 0.f && a.prm.lp_alpha <= 1.f;
+  // streams dealt round-robin over the CTAs, as in dexr_sequences_kernel.  A warp whose first group has no stream skips the
+  // round (warp-uniform: its other group's stream number is larger) instead of walking stream S - 1 for nothing and taking
+  // issue slots from the warps that have one.
+  const int first_slot = a.spw == GPW ? warp * GPW : warp;
+  for (long long base = 0; base < a.S; base += (long long)gridDim.x * kEvalWarps * a.spw) {
+    if (base + (long long)first_slot * gridDim.x + blockIdx.x >= a.S) continue;
+    const long long s = base + (long long)slot * gridDim.x + blockIdx.x;
+    vjp_stream(sv, a.io, a.dm, a.S, a.steps, s, owner && s < a.S, use_filter);
   }
 }
 
@@ -569,6 +643,8 @@ size_t dexr_frames_sizeof(void) { return sizeof(dexr_frames_t); }
 size_t dexr_sequences_sizeof(void) { return sizeof(dexr_sequences_t); }
 size_t dexr_eval_sizeof(void) { return sizeof(dexr_eval_t); }
 size_t dexr_vjp_sizeof(void) { return sizeof(dexr_vjp_t); }
+size_t dexr_sequences_tape_sizeof(void) { return sizeof(dexr_sequences_tape_t); }
+size_t dexr_sequences_vjp_sizeof(void) { return sizeof(dexr_sequences_vjp_t); }
 
 void dexr_default_params(dexr_params_t* p) {
   p->huber_delta = 0.02f;
@@ -1044,7 +1120,7 @@ extern "C" int dexr_solve_frames(const dexr_robot_t* robot, const dexr_params_t*
 
 template <int G, int BW>
 static int launch_sequences(dexr_robot* r, const dexr_params_t* prm, const dexr_sequences_t* io, long long S, int steps,
-                            cudaStream_t stream) {
+                            cudaStream_t stream, const dexr_sequences_tape_t* tape = nullptr) {
   const dexr_table_t& t = r->host;
   SeqArgs a{};
   a.table = r->table_dev;
@@ -1058,7 +1134,9 @@ static int launch_sequences(dexr_robot* r, const dexr_params_t* prm, const dexr_
   const int groups = kSeqNW * GPW;
   const int smem = a.scratch_off + groups * Scratch<G, BW>::kStreamFloats * 4;
   auto kern = dexr_sequences_kernel<G, BW, kSeqNW>;
-  CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  auto kern_tape = dexr_sequences_tape_kernel<G, BW, kSeqNW>;
+  if (tape) CUDA_TRY(cudaFuncSetAttribute(kern_tape, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  else CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
   // A stream is serial in time and latency bound, so streams are spread over as many warps and SMs as there are: while one
   // warp per stream fits into one wave of CTAs (S <= SMs x warps per CTA), a warp carries ONE stream (the second group of a
   // 16-lane solver idles); beyond that two 16-lane streams share a warp.  One CTA per SM, two when streams are plentiful.
@@ -1071,7 +1149,8 @@ static int launch_sequences(dexr_robot* r, const dexr_params_t* prm, const dexr_
   const long long per_cta = (long long)kSeqNW * a.spw;
   const long long ctas = std::max<long long>(1, (S + a.spw - 1) / a.spw);  // at least one warp's worth of streams per CTA
   int grid = (int)std::min<long long>(ctas, (long long)r->num_sms * (S >= (long long)r->num_sms * per_cta * 2 ? 2 : 1));
-  kern<<<grid, kSeqNW * 32, smem, stream>>>(a);
+  if (tape) kern_tape<<<grid, kSeqNW * 32, smem, stream>>>(a, *tape);
+  else kern<<<grid, kSeqNW * 32, smem, stream>>>(a);
   CUDA_TRY(cudaGetLastError());
   {
     std::lock_guard<std::mutex> lk(r->info_mu);
@@ -1093,6 +1172,78 @@ extern "C" int dexr_solve_sequences(const dexr_robot_t* robot, const dexr_params
   return with_solver(solver_kind(r->host, arrow_enabled()), [&](auto s) {
     return launch_sequences<decltype(s)::G, decltype(s)::BW>(r, params, io, num_streams, (int)num_steps, stream);
   });
+}
+
+extern "C" int dexr_solve_sequences_tape(const dexr_robot_t* robot, const dexr_params_t* params, const dexr_sequences_t* io,
+                                         const dexr_sequences_tape_t* tape, int64_t num_streams, int64_t num_steps,
+                                         void* cuda_stream) {
+  if (!robot || !params || !io || !tape) return fail(DEXR_E_INVALID, "dexr_solve_sequences_tape: null argument");
+  if (num_streams < 0 || num_steps < 0 || num_steps > INT32_MAX) return fail(DEXR_E_INVALID, "bad sizes");
+  if (num_streams == 0 || num_steps == 0) return 0;
+  if (int e = check_params(params)) return e;
+  if (int e = check_sequences_io(robot->host, io, params)) return e;
+  if (!tape->qpos) return fail(DEXR_E_INVALID, "tape->qpos is required");
+  if (robot->host.loss == DEXR_LOSS_DEXPILOT && (!tape->projected || !io->projected))
+    return fail(DEXR_E_INVALID, "DexPilot: the flag tape needs tape->projected and io->projected");
+  DEVICE_SCOPE(robot->device);
+  dexr_robot* r = const_cast<dexr_robot*>(robot);
+  cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
+  const dexr_sequences_tape_t tp{tape->qpos, robot->host.loss == DEXR_LOSS_DEXPILOT ? tape->projected : nullptr};
+  return with_solver(solver_kind(r->host, arrow_enabled()), [&](auto s) {
+    return launch_sequences<decltype(s)::G, decltype(s)::BW>(r, params, io, num_streams, (int)num_steps, stream, &tp);
+  });
+}
+
+// Launch shape of the sequence VJP: the VJP kernel's CTA (kEvalWarps warps, as many CTAs per SM as are resident, one wave
+// that strides over the streams), one stream per group of G lanes (two per warp for 16-lane robots: 12-14 % faster than
+// one on H100, DESIGN.md section 3.9).  DEXR_SEQ_VJP_SPW=1 (read per call) gives every 16-lane stream a warp of its own and
+// DEXR_EVAL_CTAS_PER_SM caps the CTAs per SM, for A/B runs.
+template <int G>
+static int launch_seq_vjp(dexr_robot* r, const dexr_params_t* prm, const dexr_sequences_vjp_t* io, long long S, int steps,
+                          cudaStream_t stream) {
+  const dexr_table_t& t = r->host;
+  SeqVjpArgs a{};
+  a.table = r->table_dev;
+  a.prm = sequence_params(*prm);
+  a.io = *io;
+  a.S = S;
+  a.steps = steps;
+  a.dm = make_dims(t);
+  a.scratch_off = round_up((int)sizeof(SharedTable), 16);
+  constexpr int GPW = 32 / G;
+  a.spw = GPW;
+  if (const char* e = getenv("DEXR_SEQ_VJP_SPW"))
+    if (atoi(e) == 1) a.spw = 1;
+  const int smem = a.scratch_off + kEvalWarps * GPW * VjpScratch<G>::kFloats * 4;
+  auto kern = dexr_seq_vjp_kernel<G>;
+  CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  int per_sm = 1;
+  if (int e = eval_ctas_per_sm(kern, smem, &per_sm)) return e;
+  // a stream is serial in time: deal the streams over as many CTAs as are resident (a warp's worth per CTA at least), so
+  // that a few hundred streams still reach every SM; the warps left without a stream skip the round
+  const long long ctas = (S + a.spw - 1) / a.spw;
+  const int grid = (int)std::min<long long>(ctas, (long long)r->num_sms * per_sm);
+  kern<<<grid, kEvalWarps * 32, smem, stream>>>(a);
+  CUDA_TRY(cudaGetLastError());
+  {
+    std::lock_guard<std::mutex> lk(r->info_mu);
+    r->last = dexr_launch_info_t{grid, kEvalWarps * 32, smem, 0, G, kEvalWarps, r->last.kernels_launched + 1};
+  }
+  return 0;
+}
+
+extern "C" int dexr_solve_sequences_vjp(const dexr_robot_t* robot, const dexr_params_t* params, const dexr_sequences_vjp_t* io,
+                                        int64_t num_streams, int64_t num_steps, void* cuda_stream) {
+  if (!robot || !params || !io) return fail(DEXR_E_INVALID, "dexr_solve_sequences_vjp: null argument");
+  if (num_streams < 0 || num_steps < 0 || num_steps > INT32_MAX) return fail(DEXR_E_INVALID, "bad sizes");
+  if (const char* msg = seq_vjp_io_error(robot->host, *io, *params)) return fail(DEXR_E_INVALID, "%s", msg);
+  if (int e = check_loss_params(params)) return e;
+  if (num_streams == 0 || num_steps == 0) return 0;
+  DEVICE_SCOPE(robot->device);
+  dexr_robot* r = const_cast<dexr_robot*>(robot);
+  cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
+  return eval_lanes(r->host) == 16 ? launch_seq_vjp<16>(r, params, io, num_streams, (int)num_steps, stream)
+                                   : launch_seq_vjp<32>(r, params, io, num_streams, (int)num_steps, stream);
 }
 
 extern "C" {

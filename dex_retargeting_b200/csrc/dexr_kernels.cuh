@@ -1499,10 +1499,13 @@ inline dexr_params_t sequence_params(dexr_params_t p) {
 // it on stream S - 1, and only a group that `writes` stores results and state.  `use_filter`: prm.lp_alpha in [0, 1].
 // dm, prm, S and steps are the kernel argument's and `use_filter` is computed once per thread: taken by value here, or
 // recomputed per stream, they change the register allocation of the sequences kernels.
-template <int G, int BW>
+// REC (dexr_solve_sequences_tape): the writing group also stores every frame's unfiltered solution to `tape_qpos` and, for
+// DexPilot, the flags the frame left to `tape_proj` -- two extra stores on the same code path, so the results do not change.
+template <int G, int BW, bool REC = false>
 __device__ __forceinline__ void solve_stream(Solver<G, BW>& sv, const dexr_sequences_t& io, const Dims& dm,
                                              const dexr_params_t& prm, const long long& S, const int& steps, long long s,
-                                             bool active, bool writes, float* kpbuf, bool use_filter) {
+                                             bool active, bool writes, float* kpbuf, bool use_filter,
+                                             float* tape_qpos = nullptr, uint8_t* tape_proj = nullptr) {
   constexpr int KPL = (3 * DEXR_NUM_KEYPOINTS + G - 1) / G;  // keypoint floats per lane
   const int l = sv.l;
   const long long sc = active ? s : S - 1;
@@ -1543,6 +1546,13 @@ __device__ __forceinline__ void solve_stream(Solver<G, BW>& sv, const dexr_seque
     sv.x = last;
     const int status = sv.solve(in, active);
     last = sv.x;  // unfiltered solution is the next warm start (seq_retarget.py:124)
+    if constexpr (REC) {
+      if (writes) {  // (lane l < len_proj wrote flag l of the stream's buffer in prepare_targets)
+        const long long fr = sc * steps + t;
+        if (sv.var >= 0) tape_qpos[fr * dm.n_var + sv.var] = last;
+        if (tape_proj && l < dm.len_proj) tape_proj[fr * dm.len_proj + l] = io.projected[sc * dm.len_proj + l];
+      }
+    }
     float out = sv.q;
     if (use_filter) {  // optimizer_utils.py:7-13
       fy = finit ? fmaf(prm.lp_alpha, out - fy, fy) : out;
@@ -1768,11 +1778,22 @@ __device__ __forceinline__ void vjp_column(const Solver<G, 0>& sv, int k, float&
   }
 }
 
-// One frame of dexr_solve_vjp (see dexr.h): reads qpos, grad_qpos and the frame's inputs, writes the requested cotangents
-// and the status.  `dm` is the kernel argument's, as in evaluate_frame.
+// What vjp_core hands back to its driver, per lane: v (H_ff^-1 gbar_f on this lane's variable, 0 elsewhere), the fixed-joint
+// term H_q[c, :] . M v of a fixed lane (its cotangent is -qbar), and the frame's finite / not-positive-definite verdicts
+// (group-uniform).  The keypoint cotangents are in the scratch's kKp accumulator.
+struct VjpLane {
+  float v, qbar;
+  bool finite, bad;
+};
+
+// The per-frame core of the implicit-function VJP, shared by vjp_frame (dexr_solve_vjp) and vjp_stream
+// (dexr_solve_sequences_vjp): the point x, the anchor x0 and the cotangent gbar of this lane's variable come from the driver,
+// with norm_delta `nd` (0: no regulariser) and the frame's DexPilot flags `proj` (read into the scratch; nullptr = all 0).
+// Writes the ref_value cotangents to `grad_ref` ([m,3] of the frame, or nullptr) itself; everything else goes back to the
+// driver.  The caller's flags are never written.
 template <int G>
-__device__ __forceinline__ void vjp_frame(Solver<G, 0>& sv, const FrameInputs& in_, const dexr_vjp_t& io, const Dims& dm,
-                                          long long f, bool active) {
+__device__ __forceinline__ VjpLane vjp_core(Solver<G, 0>& sv, const FrameInputs& in_, const Dims& dm, float x, float x0,
+                                            float gbar, float nd, const uint8_t* proj, float* grad_ref, bool active) {
   using VS = VjpScratch<G>;
   constexpr int NP = G;
   const SharedTable& st = Solver<G, 0>::ST();
@@ -1784,17 +1805,11 @@ __device__ __forceinline__ void vjp_frame(Solver<G, 0>& sv, const FrameInputs& i
   float* const kpacc = sv.scf() + VS::kKp;
   uint8_t* const flags = reinterpret_cast<uint8_t*>(sv.scf() + VS::kFlags);
 
-  // ---- inputs, targets (flags on the private copy), FK at x
-  float x = 0.f, x0 = 0.f, gbar = 0.f;
-  if (active && isvar) {
-    x = io.qpos[f * dm.n_var + sv.var];
-    x0 = io.last_qpos ? io.last_qpos[f * dm.n_var + sv.var] : x;
-    gbar = io.grad_qpos[f * dm.n_var + sv.var];
-  }
+  // ---- targets (flags on the private copy), FK at x
   const int fixedi = st.fixed_index[l];
   sv.qfix = (active && fixedi >= 0) ? in_.fixed[fixedi] : 0.f;
   sv.x = x;
-  if (l < dm.len_proj) flags[l] = (active && io.projected) ? io.projected[f * dm.len_proj + l] : (uint8_t)0;
+  if (l < dm.len_proj) flags[l] = (active && proj) ? proj[l] : (uint8_t)0;
   for (int e = l; e < 64; e += G) kpacc[e] = 0.f;
   __syncwarp();
   FrameInputs in = in_;
@@ -1814,7 +1829,6 @@ __device__ __forceinline__ void vjp_frame(Solver<G, 0>& sv, const FrameInputs& i
   __syncwarp();
 
   // ---- gradient of F and H_q, one residual per pass: loss curvature J^T (d2h/dr2) J, then the kinematic curvature
-  const float nd = io.last_qpos ? sv.prm.norm_delta : 0.f;  // no anchor: no regulariser
   const float beta = sv.prm.huber_delta, inv_beta = sv.inv_beta;
   const bool pos_loss = dm.loss == DEXR_LOSS_POSITION;
   float H[NP];
@@ -2005,23 +2019,143 @@ __device__ __forceinline__ void vjp_frame(Solver<G, 0>& sv, const FrameInputs& i
         kpacc[3 * ht + l] += cl;
         if (ho >= 0) kpacc[3 * ho + l] -= cl;
       }
-    } else if (active && io.grad_ref_value && l < 3) {
-      io.grad_ref_value[(f * m + k) * 3 + l] = out(cl);
+    } else if (active && grad_ref && l < 3) {
+      grad_ref[k * 3 + l] = out(cl);
     }
   }
-  // ---- fixed joints: q_bar_c = -H_q[c, :] . M v; anchor: a_bar = 2 norm_delta v
+  // ---- fixed joints: q_bar_c = -H_q[c, :] . M v (the anchor's a_bar = 2 norm_delta v is the driver's)
   float qbar = 0.f;
   if (fixedi >= 0)
     for (int i = 0; i < dof; ++i) qbar = fmaf(hq[i * NP + l], mvs[i], qbar);
   __syncwarp();
+  return VjpLane{v, qbar, finite, bad};
+}
+
+// One frame of dexr_solve_vjp (see dexr.h): reads qpos, grad_qpos and the frame's inputs, writes the requested cotangents
+// and the status.  `dm` is the kernel argument's, as in evaluate_frame.
+template <int G>
+__device__ __forceinline__ void vjp_frame(Solver<G, 0>& sv, const FrameInputs& in, const dexr_vjp_t& io, const Dims& dm,
+                                          long long f, bool active) {
+  const int l = sv.l;
+  const bool isvar = sv.var >= 0;
+  float x = 0.f, x0 = 0.f, gbar = 0.f;
+  if (active && isvar) {
+    x = io.qpos[f * dm.n_var + sv.var];
+    x0 = io.last_qpos ? io.last_qpos[f * dm.n_var + sv.var] : x;
+    gbar = io.grad_qpos[f * dm.n_var + sv.var];
+  }
+  const float nd = io.last_qpos ? sv.prm.norm_delta : 0.f;  // no anchor: no regulariser
+  const VjpLane r = vjp_core(sv, in, dm, x, x0, gbar, nd, io.projected ? io.projected + f * dm.len_proj : nullptr,
+                             io.grad_ref_value ? io.grad_ref_value + f * dm.n_res * 3 : nullptr, active);
+  const int fixedi = Solver<G, 0>::ST().fixed_index[l];
+  const bool by_kp = in.kp != nullptr;
+  const float* const kpacc = sv.scf() + VjpScratch<G>::kKp;
+  // outputs: NaN for a frame with a non-finite input, 0 for one whose free Hessian is not positive definite
+  auto out = [&](float val) { return !r.finite ? __int_as_float(0x7fc00000) : (r.bad ? 0.f : val); };
   if (active) {
-    if (isvar && io.grad_last_qpos) io.grad_last_qpos[f * dm.n_var + sv.var] = out(2.0f * nd * v);
-    if (fixedi >= 0 && io.grad_fixed_qpos) io.grad_fixed_qpos[f * dm.n_fixed + fixedi] = out(-qbar);
+    if (isvar && io.grad_last_qpos) io.grad_last_qpos[f * dm.n_var + sv.var] = out(2.0f * nd * r.v);
+    if (fixedi >= 0 && io.grad_fixed_qpos) io.grad_fixed_qpos[f * dm.n_fixed + fixedi] = out(-r.qbar);
     if (by_kp && io.grad_keypoints)
       for (int e = l; e < 3 * DEXR_NUM_KEYPOINTS; e += G) io.grad_keypoints[f * 3 * DEXR_NUM_KEYPOINTS + e] = out(kpacc[e]);
-    if (l == 0 && io.status_out) io.status_out[f] = !finite ? DEXR_STATUS_NONFINITE : (bad ? DEXR_STATUS_NOT_PD : 0);
+    if (l == 0 && io.status_out) io.status_out[f] = !r.finite ? DEXR_STATUS_NONFINITE : (r.bad ? DEXR_STATUS_NOT_PD : 0);
   }
   __syncwarp();  // the group's next frame rewrites the scratch this one read
+}
+
+// ------------------------------------------------------------------------------------------------
+// backpropagation through the sequence solve (dexr_solve_sequences_vjp): the reverse-time recurrence of a stream
+// ------------------------------------------------------------------------------------------------
+// The argument checks of dexr_solve_sequences_vjp that read the robot's table or the parameters: nullptr, or what is wrong.
+// Host code shared by the library and the host emulation, as vjp_io_error.
+inline const char* seq_vjp_io_error(const dexr_table_t& t, const dexr_sequences_vjp_t& io, const dexr_params_t& prm) {
+  if (prm.preprocess != 0) return "raw-landmark pre-processing is not differentiated: params.preprocess must be 0";
+  if (!io.qpos) return "qpos (the tape of the forward call) is required";
+  if (!io.last_qpos) return "last_qpos (the warm start before the forward call) is required";
+  if (!io.keypoints) return "keypoints are required";
+  const bool use_filter = prm.lp_alpha >= 0.f && prm.lp_alpha <= 1.f;
+  if (use_filter && !io.filter_init) return "the low-pass filter needs filter_init (as before the forward call)";
+  if (t.loss == DEXR_LOSS_DEXPILOT && !io.projected) return "DexPilot needs the flag tape (projected)";
+  if (t.n_fixed > 0 && !io.fixed_qpos) return "the robot has fixed joints but fixed_qpos is NULL";
+  return nullptr;
+}
+
+// One stream s of S, walked from its last frame to its first (dexr.h, dexr_solve_sequences_vjp): gy (the filter's cotangent,
+// lane = joint) and c (the anchor cotangent flowing to the previous solution, lane = variable) stay in registers between
+// frames; each frame runs vjp_core at (x_t, clip(x_{t-1})) with gbar = M^T gq + c.  A group that is not `active` walks
+// stream S - 1 and writes nothing.  `dm`, S and steps are the kernel argument's, as in solve_stream.
+template <int G>
+__device__ __forceinline__ void vjp_stream(Solver<G, 0>& sv, const dexr_sequences_vjp_t& io, const Dims& dm, const long long& S,
+                                           const int& steps, long long s, bool active, bool use_filter) {
+  const SharedTable& st = Solver<G, 0>::ST();
+  const int l = sv.l;
+  const bool isvar = sv.var >= 0, isjoint = l < dm.dof;
+  const long long sc = active ? s : S - 1;
+  const float alpha = sv.prm.lp_alpha, nd = sv.prm.norm_delta;
+  float gy = 0.f, c = 0.f;
+  if (active && isjoint && io.grad_filter_state_out) gy = io.grad_filter_state_out[sc * dm.dof + l];
+  if (active && isvar && io.grad_last_qpos_out) c = io.grad_last_qpos_out[sc * dm.n_var + sv.var];
+  const bool finit = active && use_filter && io.filter_init[sc];
+  for (int t = steps - 1; t >= 0; --t) {
+    const long long fr = sc * steps + t;
+    // dl/dq_t of this lane's joint: the output's cotangent, through the filter (y_t = y_{t-1} + alpha (q_t - y_{t-1}))
+    float gq = (active && isjoint && io.grad_robot_qpos) ? io.grad_robot_qpos[fr * dm.dof + l] : 0.f;
+    if (use_filter) {
+      gy += gq;
+      const bool init = t > 0 || finit;
+      gq = init ? alpha * gy : gy;
+      gy = init ? (1.0f - alpha) * gy : 0.f;
+    }
+    // gbar = M^T gq on the variables (mimic followers folded into their source, as in evaluate_frame) + the anchor cotangent
+    float gbar = gq;
+    if (dm.has_mimic) {
+      const int gcount = st.group_count[l];
+      float gx_ = 0.f;
+#pragma unroll
+      for (int k = 0; k < DEXR_MAX_GROUP; ++k) {
+        const bool v = isvar && k < gcount;
+        const float gv = gshfl<G>(gq, v ? st.group_lane[l][k] : l);
+        if (v) gx_ = fmaf(st.group_mult[l][k], gv, gx_);
+      }
+      gbar = gx_;
+    }
+    gbar = isvar ? gbar + c : 0.f;
+    // the point x_t and the anchor a_t = clip(x_{t-1}) the forward solved from
+    float x = 0.f, xp = 0.f;
+    if (active && isvar) {
+      x = io.qpos[fr * dm.n_var + sv.var];
+      xp = t > 0 ? io.qpos[(fr - 1) * dm.n_var + sv.var] : io.last_qpos[sc * dm.n_var + sv.var];
+    }
+    const float clo = st.clip_lo[l], chi = st.clip_hi[l];
+    const float a = fminf(fmaxf(xp, clo), chi);
+    const bool passes = xp >= clo && xp <= chi;  // the clip passes the anchor's cotangent (inclusive bounds, as torch.clamp)
+    FrameInputs in;
+    in.kp = io.keypoints + fr * (3 * DEXR_NUM_KEYPOINTS);
+    in.ref = nullptr;
+    in.fixed = dm.n_fixed > 0 ? io.fixed_qpos + fr * dm.n_fixed : nullptr;
+    in.last = nullptr;
+    in.projected = nullptr;
+    const VjpLane r = vjp_core(sv, in, dm, x, a, gbar, nd, io.projected ? io.projected + fr * dm.len_proj : nullptr,
+                               nullptr, active);
+    // outputs: NaN for a frame with a non-finite input (and, through c, for every earlier frame of the stream); v = 0 for
+    // one whose free Hessian is not positive definite
+    auto out = [&](float val) { return !r.finite ? __int_as_float(0x7fc00000) : val; };
+    // the anchor's cotangent reaches x_{t-1} where the clip passes it; NaN stays NaN
+    c = out(2.0f * nd * r.v) * (passes ? 1.0f : 0.f);
+    if (active) {
+      const int fixedi = st.fixed_index[l];
+      const float* const kpacc = sv.scf() + VjpScratch<G>::kKp;
+      if (fixedi >= 0 && io.grad_fixed_qpos) io.grad_fixed_qpos[fr * dm.n_fixed + fixedi] = out(gq - r.qbar);
+      if (io.grad_keypoints)
+        for (int e = l; e < 3 * DEXR_NUM_KEYPOINTS; e += G) io.grad_keypoints[fr * 3 * DEXR_NUM_KEYPOINTS + e] = out(kpacc[e]);
+      if (l == 0 && io.status_out) io.status_out[fr] = !r.finite ? DEXR_STATUS_NONFINITE : (r.bad ? DEXR_STATUS_NOT_PD : 0);
+    }
+    __syncwarp();  // the next frame rewrites the scratch this one read
+  }
+  if (active) {
+    if (isvar && io.grad_last_qpos) io.grad_last_qpos[sc * dm.n_var + sv.var] = c;
+    if (isjoint && io.grad_filter_state)  // (without a filter gy is still the incoming cotangent: the state passes through)
+      io.grad_filter_state[sc * dm.dof + l] = gy;
+  }
 }
 
 }  // namespace dexr

@@ -9,6 +9,11 @@ or the anchor are not computed: those arguments must not require grad.
 `differentiable_retarget(opt, ...)` is the other direction: the solve's answer as a differentiable function of the keypoints
 (or ref_value), the fixed joints and the anchor (`Optimizer.retarget_batch` forward, `Optimizer.retarget_batch_vjp` backward):
 a hand-pose network trained with a loss on the robot joint angles backpropagates through the retargeting with it.
+
+`differentiable_retarget_sequences(seq, keypoints, state)` does the same for whole streams with `SeqRetargeting`'s
+semantics (clipped warm start, carried solution, mimic, low-pass filter): forward one recorded `retarget_sequences` launch,
+backward one `retarget_sequences_vjp` launch through every frame of every stream.  The returned state carries the graph,
+so chained calls backpropagate across chunk boundaries.
 """
 from __future__ import annotations
 
@@ -90,3 +95,62 @@ def differentiable_retarget(opt, *, keypoints=None, ref_value=None, fixed_qpos=N
                          "(dexr_preprocess_keypoints) and pass them without raw_hand")
     cfg = dict(by_kp=keypoints is not None, projected=projected, clip_init=clip_init, raw_hand=raw_hand)
     return _DifferentiableRetarget.apply(targets, fixed_qpos, last_qpos, opt, cfg)
+
+
+class _DifferentiableRetargetSequences(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, keypoints, fixed_qpos, last_qpos, filter_state, seq, cfg):
+        from .seq_retarget import StreamState
+
+        st = cfg["state"]
+        new = StreamState(last_qpos=last_qpos.detach().clone(), filter_state=filter_state.detach().clone(),
+                          filter_init=st.filter_init.clone(), projected=None if st.projected is None else st.projected.clone(),
+                          damping=None if st.damping is None else st.damping.clone())
+        S, T = int(keypoints.shape[0]), int(keypoints.shape[1])
+        tape = seq.make_sequence_tape(S, T)
+        kp = keypoints.detach().contiguous()
+        fixed = None if fixed_qpos is None else fixed_qpos.detach().contiguous()
+        out, _ = seq.retarget_sequences(kp, new, fixed_qpos=fixed, tape=tape)
+        ctx.seq, ctx.tape = seq, tape
+        ctx.save_for_backward(kp, fixed, last_qpos.detach().contiguous(), st.filter_init.clone())
+        ctx.set_materialize_grads(False)
+        cfg["new_state"] = new
+        return out, new.last_qpos, new.filter_state
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g_out, g_last, g_filter):
+        keypoints, fixed, last0, finit0 = ctx.saved_tensors
+        c = (lambda g: None if g is None else g.contiguous())
+        g_kp, g_fixed, g_last0, g_filter0 = ctx.seq.retarget_sequences_vjp(
+            keypoints, ctx.tape, last0, finit0, grad_robot_qpos=c(g_out), grad_last_qpos=c(g_last),
+            grad_filter_state=c(g_filter), fixed_qpos=fixed)
+        return g_kp, g_fixed, g_last0, g_filter0, None, None
+
+
+def differentiable_retarget_sequences(seq, keypoints, state=None, fixed_qpos=None, *, raw_hand=None):
+    """(robot_qpos [S,T,dof], new_state) = `seq.retarget_sequences(keypoints, state, fixed_qpos)` (float32 CUDA tensors as
+    there), differentiable in `keypoints`, `fixed_qpos`, `state.last_qpos` and `state.filter_state`.  `state` (None: fresh
+    streams, `seq.make_stream_state`) is not modified: autograd keeps it, and a new `StreamState` comes back whose
+    `last_qpos` and `filter_state` carry the graph -- feed it to the next call for full or truncated (detach it)
+    backpropagation through time over long recordings.  backward() is one `retarget_sequences_vjp` launch: every frame's
+    implicit-function derivative at its solution and clipped anchor, the anchor chain through the clip and the low-pass
+    filter (see `SeqRetargeting.retarget_sequences_vjp`).  Raw detector landmarks (`raw_hand`) are solved but not
+    differentiated: pre-process them first."""
+    from .seq_retarget import StreamState
+
+    S = int(keypoints.shape[0])
+    state = seq.make_stream_state(S) if state is None else state
+    if raw_hand is not None:
+        if any(t is not None and t.requires_grad for t in (keypoints, fixed_qpos, state.last_qpos, state.filter_state)):
+            raise ValueError("raw_hand: raw-landmark pre-processing is not differentiated; pre-process the keypoints "
+                             "(dexr_preprocess_keypoints) and pass them without raw_hand")
+        new = StreamState(**{k: (None if getattr(state, k) is None else getattr(state, k).clone()) for k in StreamState._FIELDS})
+        out, new = seq.retarget_sequences(keypoints, new, fixed_qpos=fixed_qpos, raw_hand=raw_hand)
+        return out, new
+    cfg = dict(state=state)
+    out, last, filt = _DifferentiableRetargetSequences.apply(keypoints, fixed_qpos, state.last_qpos, state.filter_state, seq,
+                                                             cfg)
+    new = cfg["new_state"]
+    return out, StreamState(last_qpos=last, filter_state=filt, filter_init=new.filter_init, projected=new.projected,
+                            damping=new.damping)

@@ -8,6 +8,9 @@ pinocchio-ordered qpos, applies mimic joints and the low-pass filter, returns fl
 New, batched: `retarget_sequences()` runs S independent streams x T frames with exactly that recurrence
 inside ONE kernel launch (`dexr_solve_sequences`): a group of lanes owns a stream and walks its frames,
 `last_qpos`, the DexPilot hysteresis flags and the filter state never leave the SM between frames.
+With a `SequenceTape` the same launch also records every frame's unfiltered solution (and DexPilot flags), and
+`retarget_sequences_vjp()` backpropagates through all T frames of every stream in one launch
+(`dexr_solve_sequences_vjp`; `objective.differentiable_retarget_sequences` wraps both for autograd).
 """
 from __future__ import annotations
 
@@ -64,6 +67,15 @@ class StreamState:
         if st.damping is None:
             st.damping = torch.zeros((S,), dtype=torch.float32, device=st.last_qpos.device)
         return st
+
+
+@dataclass
+class SequenceTape:
+    """What a recorded `retarget_sequences` call leaves for its backward (`dexr_sequences_tape_t`): torch tensors on the
+    optimizer's device."""
+
+    qpos: "torch.Tensor"                 # [S, T, opt_dof] float32: every frame's unfiltered solution
+    projected: Optional["torch.Tensor"]  # [S, T, len_proj] uint8: the DexPilot flags after every frame, or None
 
 
 def _quat_to_matrix(q):
@@ -250,13 +262,30 @@ class SeqRetargeting:
             damping=torch.zeros((num_streams,), dtype=torch.float32, device=dev),
         )
 
+    def make_sequence_tape(self, num_streams: int, num_steps: int) -> SequenceTape:
+        """Empty tape buffers for a recorded `retarget_sequences` call of S streams x T frames."""
+        import torch
+
+        opt = self.optimizer
+        dev = torch.device("cuda", opt.device_index)
+        len_proj = opt._objective_spec().len_proj
+        return SequenceTape(
+            qpos=torch.empty((num_streams, num_steps, opt.opt_dof), dtype=torch.float32, device=dev),
+            projected=(torch.empty((num_streams, num_steps, len_proj), dtype=torch.uint8, device=dev)
+                       if opt.retargeting_type == "DEXPILOT" else None))
+
     def retarget_sequences(self, keypoints, state: Optional[StreamState] = None, fixed_qpos=None, out=None,
-                           status_out=None, stream=None, raw_hand=None):
+                           status_out=None, stream=None, raw_hand=None, tape: Optional[SequenceTape] = None):
         """keypoints: float32 CUDA tensor [S,T,21,3] (raw 21-point hand frames).  Runs every stream
         through T SeqRetargeting.retarget() steps in one launch.  Returns (robot_qpos [S,T,dof] float32
         in pinocchio joint order, filtered; state) -- `state` is updated in place and can be passed
         to the next call to continue the streams.  `raw_hand` (HandType): the keypoints are raw detector landmarks of that
-        hand, pre-processed inside the kernel (Optimizer.params)."""
+        hand, pre-processed inside the kernel (Optimizer.params).
+        `tape` (`make_sequence_tape(S, T)`): the same launch also records what `retarget_sequences_vjp` needs
+        (`dexr_solve_sequences_tape`); the results are bit-identical to an unrecorded call."""
+        if tape is not None and raw_hand is not None:
+            raise ValueError("raw_hand with a tape: raw-landmark pre-processing is not differentiated; pre-process the "
+                             "keypoints (dexr_preprocess_keypoints) and record the call without raw_hand")
         import torch
 
         opt = self.optimizer
@@ -295,6 +324,79 @@ class SeqRetargeting:
             io.status_out = chk(status_out, (S, T), torch.int32, "status_out")
         s = stream if stream is not None else torch.cuda.current_stream(dev)
         p = opt.params(clip_init=True, lp_alpha=self.low_pass_alpha, raw_hand=raw_hand)
-        N.check(eng.lib.dexr_solve_sequences(eng.handle, C.byref(p), C.byref(io), S, T, C.c_void_p(s.cuda_stream)),
-                "dexr_solve_sequences")
+        if tape is None:
+            N.check(eng.lib.dexr_solve_sequences(eng.handle, C.byref(p), C.byref(io), S, T, C.c_void_p(s.cuda_stream)),
+                    "dexr_solve_sequences")
+            return out, state
+        tp = N.DexrSequencesTape()
+        tp.qpos = chk(tape.qpos, (S, T, opt.opt_dof), torch.float32, "tape.qpos")
+        if tape.projected is not None:
+            tp.projected = chk(tape.projected, (S, T, opt._objective_spec().len_proj), torch.uint8, "tape.projected")
+        N.check(eng.lib.dexr_solve_sequences_tape(eng.handle, C.byref(p), C.byref(io), C.byref(tp), S, T,
+                                                  C.c_void_p(s.cuda_stream)), "dexr_solve_sequences_tape")
         return out, state
+
+    def retarget_sequences_vjp(self, keypoints, tape: SequenceTape, last_qpos0, filter_init0, grad_robot_qpos=None,
+                               grad_last_qpos=None, grad_filter_state=None, fixed_qpos=None, grad_keypoints_out=None,
+                               grad_fixed_qpos_out=None, grad_last_qpos_out=None, grad_filter_state_out=None,
+                               status_out=None, stream=None):
+        """Backpropagate through a recorded `retarget_sequences(keypoints, state, fixed_qpos, tape=tape)` call, one launch
+        (`dexr_solve_sequences_vjp`).  `last_qpos0` [S,opt_dof] and `filter_init0` [S] uint8 are the state's `last_qpos` and
+        `filter_init` as they were BEFORE that call; the cotangents are dl/drobot_qpos [S,T,dof] (`grad_robot_qpos`) and
+        dl/d the final `state.last_qpos` / `state.filter_state` (`grad_last_qpos`, `grad_filter_state`), each None for 0.
+        Returns (grad_keypoints [S,T,21,3], grad_fixed_qpos [S,T,n_fixed] or None, grad_last_qpos0 [S,opt_dof],
+        grad_filter_state0 [S,dof]): the gradients with respect to the call's keypoints, fixed joints and initial state.
+        Every frame is differentiated as by `Optimizer.retarget_batch_vjp` at its recorded solution and clipped anchor;
+        the DexPilot flags, the carried damping and the basin the warm start picks are not differentiated.  `status_out`
+        [S,T] int32 receives 0, STATUS_NONFINITE (this frame or a later one of the stream is non-finite: NaN outputs) or
+        STATUS_NOT_PD (zero cotangents through the solve).  Keypoints must not be raw landmarks.  Nothing is synchronised."""
+        import torch
+
+        opt = self.optimizer
+        eng = opt.engine()
+        dev = torch.device("cuda", eng.device)
+        if keypoints.dim() != 4 or tuple(keypoints.shape[2:]) != (N.NUM_KEYPOINTS, 3):
+            raise ValueError(f"keypoints must have shape [S,T,21,3], got {tuple(keypoints.shape)}")
+        S, T = int(keypoints.shape[0]), int(keypoints.shape[1])
+        n, dof, nf = opt.opt_dof, opt.robot.dof, len(opt.idx_pin2fixed)
+
+        def chk(t, shape, dtype, name):
+            if t.device != dev or t.dtype != dtype or not t.is_contiguous() or tuple(t.shape) != tuple(shape):
+                raise ValueError(f"{name}: expected contiguous {dtype} tensor of shape {tuple(shape)} on {dev}, "
+                                 f"got {t.dtype} {tuple(t.shape)} on {t.device}")
+            return t.data_ptr()
+
+        def out(t, shape, name):
+            t = torch.empty(shape, dtype=torch.float32, device=dev) if t is None else t
+            return t, chk(t, shape, torch.float32, name)
+
+        io = N.DexrSequencesVjp()
+        io.keypoints = chk(keypoints, (S, T, N.NUM_KEYPOINTS, 3), torch.float32, "keypoints")
+        if nf:
+            if fixed_qpos is None:
+                raise ValueError(f"Optimizer has {nf} fixed joints but no fixed_qpos is given")
+            io.fixed_qpos = chk(fixed_qpos, (S, T, nf), torch.float32, "fixed_qpos")
+        io.last_qpos = chk(last_qpos0, (S, n), torch.float32, "last_qpos0")
+        io.filter_init = chk(filter_init0, (S,), torch.uint8, "filter_init0")
+        io.qpos = chk(tape.qpos, (S, T, n), torch.float32, "tape.qpos")
+        if tape.projected is not None:
+            io.projected = chk(tape.projected, (S, T, opt._objective_spec().len_proj), torch.uint8, "tape.projected")
+        if grad_robot_qpos is not None:
+            io.grad_robot_qpos = chk(grad_robot_qpos, (S, T, dof), torch.float32, "grad_robot_qpos")
+        if grad_last_qpos is not None:
+            io.grad_last_qpos_out = chk(grad_last_qpos, (S, n), torch.float32, "grad_last_qpos")
+        if grad_filter_state is not None:
+            io.grad_filter_state_out = chk(grad_filter_state, (S, dof), torch.float32, "grad_filter_state")
+        g_kp, io.grad_keypoints = out(grad_keypoints_out, (S, T, N.NUM_KEYPOINTS, 3), "grad_keypoints_out")
+        g_fixed = None
+        if nf:
+            g_fixed, io.grad_fixed_qpos = out(grad_fixed_qpos_out, (S, T, nf), "grad_fixed_qpos_out")
+        g_last, io.grad_last_qpos = out(grad_last_qpos_out, (S, n), "grad_last_qpos_out")
+        g_filter, io.grad_filter_state = out(grad_filter_state_out, (S, dof), "grad_filter_state_out")
+        if status_out is not None:
+            io.status_out = chk(status_out, (S, T), torch.int32, "status_out")
+        s = stream if stream is not None else torch.cuda.current_stream(dev)
+        p = opt.params(clip_init=True, lp_alpha=self.low_pass_alpha)
+        N.check(eng.lib.dexr_solve_sequences_vjp(eng.handle, C.byref(p), C.byref(io), S, T, C.c_void_p(s.cuda_stream)),
+                "dexr_solve_sequences_vjp")
+        return g_kp, g_fixed, g_last, g_filter

@@ -317,6 +317,49 @@ size_t dexr_vjp_sizeof(void);
 int dexr_solve_vjp(const dexr_robot_t* robot, const dexr_params_t* params, const dexr_vjp_t* io, int64_t num_frames,
                    void* cuda_stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Backpropagation through the sequence solve.  dexr_solve_sequences_tape is dexr_solve_sequences (same kernel code, same
+ * results bit for bit) that also records what the backward needs: every frame's UNFILTERED solution x_t and, for DexPilot,
+ * the hysteresis flags the frame left (DexPilot needs io->projected then).  dexr_solve_sequences_vjp then runs the
+ * reverse-time recurrence of every stream in one launch, a group of lanes per stream walking t = T-1 .. 0:
+ *   a_t = clip(x_{t-1}) (clip_lo / clip_hi), x_t = solve(kp_t, fixed_t, anchor a_t), q_t = scatter + mimic of x_t,
+ *   y_t = init_t ? y_{t-1} + alpha (q_t - y_{t-1}) : q_t with init_t = t > 0 or filter_init, robot_qpos[t] = y_t (or q_t);
+ * each frame is differentiated as by dexr_solve_vjp at (x_t, anchor a_t, the recorded flags), the anchor cotangent flows to
+ * x_{t-1} where clip_lo <= x_{t-1} <= clip_hi, and the filter's cotangent is carried in registers.  The DexPilot flags, the
+ * carried damping and the basin the warm start picks are not differentiated.  A frame with a non-finite input or cotangent
+ * gets non-finite outputs and DEXR_STATUS_NONFINITE, and so does every earlier frame of its stream (other streams are
+ * untouched); DEXR_STATUS_NOT_PD frames get zero cotangents and cut the chain through the anchor.  params as given to the
+ * forward (lp_alpha selects the filter, clipping is implied); params.preprocess must be 0.  Both calls are asynchronous on
+ * `cuda_stream`, allocate nothing and do nothing for 0 streams or 0 steps.  All pointers are DEVICE pointers.
+ * ------------------------------------------------------------------------------------------- */
+typedef struct dexr_sequences_tape {
+  float* qpos;        /* [S,T,n_var] every frame's unfiltered solution                      */
+  uint8_t* projected; /* [S,T,len_proj] DexPilot flags after every frame, or NULL           */
+} dexr_sequences_tape_t;
+size_t dexr_sequences_tape_sizeof(void);
+int dexr_solve_sequences_tape(const dexr_robot_t* robot, const dexr_params_t* params, const dexr_sequences_t* io,
+                              const dexr_sequences_tape_t* tape, int64_t num_streams, int64_t num_steps, void* cuda_stream);
+
+typedef struct dexr_sequences_vjp {
+  const float* keypoints;             /* [S,T,21,3] as given to the forward (preprocess must be 0)   */
+  const float* fixed_qpos;            /* [S,T,n_fixed] or NULL when n_fixed == 0                     */
+  const float* last_qpos;             /* [S,n_var] the warm start BEFORE the forward call            */
+  const uint8_t* filter_init;         /* [S] LPFilter.is_init before the forward call (filter only)  */
+  const float* qpos;                  /* [S,T,n_var] tape                                            */
+  const uint8_t* projected;           /* [S,T,len_proj] tape, DexPilot only                          */
+  const float* grad_robot_qpos;       /* [S,T,dof] or NULL (= 0)                                     */
+  const float* grad_last_qpos_out;    /* [S,n_var] dl/d final last_qpos, or NULL                     */
+  const float* grad_filter_state_out; /* [S,dof] dl/d final filter_state, or NULL                    */
+  float* grad_keypoints;              /* [S,T,21,3] or NULL                                          */
+  float* grad_fixed_qpos;             /* [S,T,n_fixed] or NULL                                       */
+  float* grad_last_qpos;              /* [S,n_var] or NULL: dl/d initial last_qpos                   */
+  float* grad_filter_state;           /* [S,dof] or NULL: dl/d initial filter_state                  */
+  int32_t* status_out;                /* [S,T] or NULL: 0, NONFINITE or NOT_PD                       */
+} dexr_sequences_vjp_t;
+size_t dexr_sequences_vjp_sizeof(void);
+int dexr_solve_sequences_vjp(const dexr_robot_t* robot, const dexr_params_t* params, const dexr_sequences_vjp_t* io,
+                             int64_t num_streams, int64_t num_steps, void* cuda_stream);
+
 #ifdef __cplusplus
 }
 #endif
