@@ -106,6 +106,16 @@ class DexrSequencesVjp(C.Structure):
     ]
 
 
+class DexrJacobian(C.Structure):
+    """Mirror of `dexr_jacobian_t`: buffers of one per-frame Jacobian launch (`dexr_solve_jacobian`)."""
+
+    _fields_ = [
+        ("keypoints", C.c_void_p), ("ref_value", C.c_void_p), ("fixed_qpos", C.c_void_p), ("qpos", C.c_void_p),
+        ("last_qpos", C.c_void_p), ("projected", C.c_void_p), ("jac_keypoints", C.c_void_p), ("jac_ref_value", C.c_void_p),
+        ("jac_fixed_qpos", C.c_void_p), ("jac_last_qpos", C.c_void_p), ("status_out", C.c_void_p),
+    ]
+
+
 class DexrGroup(C.Structure):
     """Mirror of `dexr_group_t`: one (robot, batch) group of a mixed-robot launch."""
 
@@ -127,6 +137,7 @@ EXPORTS = [
     "dexr_solve_frames", "dexr_solve_frames_multi", "dexr_solve_sequences", "dexr_solve_frames_host", "dexr_get_launch_info",
     "dexr_preprocess_keypoints", "dexr_eval_sizeof", "dexr_eval_objective", "dexr_vjp_sizeof", "dexr_solve_vjp",
     "dexr_sequences_tape_sizeof", "dexr_solve_sequences_tape", "dexr_sequences_vjp_sizeof", "dexr_solve_sequences_vjp",
+    "dexr_jacobian_sizeof", "dexr_solve_jacobian",
 ]
 
 _LIB = None
@@ -212,6 +223,14 @@ def load():
     elif not os.environ.get("DEXR_LIBRARY"):
         raise DexrError(f"{path} does not export dexr_sequences_vjp_sizeof: rebuild it "
                         "(python -m dex_retargeting_b200.build --force)")
+    if hasattr(lib, "dexr_jacobian_sizeof"):
+        lib.dexr_jacobian_sizeof.restype = C.c_size_t
+        if lib.dexr_jacobian_sizeof() != C.sizeof(DexrJacobian):
+            raise DexrError("dexr_jacobian_t layout mismatch between library and binding (stale DEXR_LIBRARY?)")
+        lib.dexr_solve_jacobian.argtypes = [C.c_void_p, C.POINTER(DexrParams), C.POINTER(DexrJacobian), C.c_int64,
+                                            C.c_void_p]
+    elif not os.environ.get("DEXR_LIBRARY"):
+        raise DexrError(f"{path} does not export dexr_jacobian_sizeof: rebuild it (python -m dex_retargeting_b200.build --force)")
     # (an older A/B library named by DEXR_LIBRARY reads a prefix of the buffer structs -- fields are only ever appended -- so
     # the single-robot entry points still work with it; dexr_solve_frames_multi, whose groups embed the struct, does not)
     _LIB = lib

@@ -356,6 +356,44 @@ __global__ void __launch_bounds__(kEvalWarps * 32, 2) dexr_vjp_kernel(const VjpA
 }
 
 // ------------------------------------------------------------------------------------------------
+// per-frame Jacobians of the solve: the VJP kernel's launch shape, one frame per group of G lanes, one tail per free variable
+// ------------------------------------------------------------------------------------------------
+struct JacobianArgs {
+  const dexr_table_t* table;
+  dexr_params_t prm;
+  dexr_jacobian_t io;
+  long long B;
+  int in_row;  // floats per frame of the kp/ref input (63 or 3m)
+  Dims dm;
+  int scratch_off;
+};
+
+template <int G>
+__global__ void __launch_bounds__(kEvalWarps * 32, 2) dexr_jacobian_kernel(const JacobianArgs a) {
+  load_shared_table(*reinterpret_cast<SharedTable*>(dsmem), a.table);  // (the residual-pass schedule is not read)
+  __syncthreads();
+  constexpr int GPW = 32 / G;
+  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
+  const int lane = threadIdx.x & 31;
+  Solver<G, 0> sv;
+  sv.init(a.table, a.dm, (uint32_t)(a.scratch_off + (warp * GPW + lane / G) * VjpScratch<G>::kFloats * 4), a.prm, lane);
+  const bool by_kp = a.io.keypoints != nullptr;
+  const long long step = (long long)gridDim.x * kEvalWarps * GPW;
+  for (long long base = ((long long)blockIdx.x * kEvalWarps + warp) * GPW; base < a.B; base += step) {
+    const long long idx = base + lane / G;
+    const bool active = idx < a.B;
+    const long long f = active ? idx : base;
+    FrameInputs in;
+    in.kp = by_kp ? a.io.keypoints + f * a.in_row : nullptr;
+    in.ref = by_kp ? nullptr : a.io.ref_value + f * a.in_row;
+    in.fixed = a.dm.n_fixed > 0 ? a.io.fixed_qpos + f * a.dm.n_fixed : nullptr;
+    in.last = nullptr;
+    in.projected = nullptr;  // (jacobian_frame reads the flags into its scratch)
+    jacobian_frame(sv, in, a.io, a.dm, f, active);
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
 // backpropagation through the sequence solve: one stream per group of G lanes, walked from its last frame to its first
 // ------------------------------------------------------------------------------------------------
 struct SeqVjpArgs {
@@ -645,6 +683,7 @@ size_t dexr_eval_sizeof(void) { return sizeof(dexr_eval_t); }
 size_t dexr_vjp_sizeof(void) { return sizeof(dexr_vjp_t); }
 size_t dexr_sequences_tape_sizeof(void) { return sizeof(dexr_sequences_tape_t); }
 size_t dexr_sequences_vjp_sizeof(void) { return sizeof(dexr_sequences_vjp_t); }
+size_t dexr_jacobian_sizeof(void) { return sizeof(dexr_jacobian_t); }
 
 void dexr_default_params(dexr_params_t* p) {
   p->huber_delta = 0.02f;
@@ -877,7 +916,7 @@ static int check_loss_params(const dexr_params_t* p) {
 // CTAs per SM of the evaluation kernel: as many as are resident at once (registers and shared memory allow), one wave that
 // grid-strides over the batch.  DEXR_EVAL_CTAS_PER_SM (read per call) caps it for A/B runs.  The choice is measured in
 // DESIGN.md section 3 ("Objective evaluation").
-// The VJP kernel uses the same rule and cap.
+// The VJP and Jacobian kernels use the same rule and cap.
 template <class K>
 static int eval_ctas_per_sm(K kern, int smem, int* out) {
   int resident = 0;
@@ -974,6 +1013,49 @@ extern "C" int dexr_solve_vjp(const dexr_robot_t* robot, const dexr_params_t* pa
   cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
   return eval_lanes(r->host) == 16 ? launch_vjp<16>(r, params, io, num_frames, stream)
                                    : launch_vjp<32>(r, params, io, num_frames, stream);
+}
+
+template <int G>
+static int launch_jacobian(dexr_robot* r, const dexr_params_t* prm, const dexr_jacobian_t* io, long long B,
+                           cudaStream_t stream) {
+  const dexr_table_t& t = r->host;
+  JacobianArgs a{};
+  a.table = r->table_dev;
+  a.prm = *prm;
+  a.io = *io;
+  a.B = B;
+  a.in_row = io->keypoints ? 3 * DEXR_NUM_KEYPOINTS : 3 * t.n_res;
+  a.dm = make_dims(t);
+  a.scratch_off = round_up((int)sizeof(SharedTable), 16);
+  constexpr int GPW = 32 / G;
+  const int smem = a.scratch_off + kEvalWarps * GPW * VjpScratch<G>::kFloats * 4;  // as the VJP kernel's
+  auto kern = dexr_jacobian_kernel<G>;
+  CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  int per_sm = 1;
+  if (int e = eval_ctas_per_sm(kern, smem, &per_sm)) return e;
+  const long long ctas = (B + kEvalWarps * GPW - 1) / (kEvalWarps * GPW);
+  const int grid = (int)std::min<long long>(ctas, (long long)r->num_sms * per_sm);
+  kern<<<grid, kEvalWarps * 32, smem, stream>>>(a);
+  CUDA_TRY(cudaGetLastError());
+  {
+    std::lock_guard<std::mutex> lk(r->info_mu);
+    r->last = dexr_launch_info_t{grid, kEvalWarps * 32, smem, 0, G, kEvalWarps, r->last.kernels_launched + 1};
+  }
+  return 0;
+}
+
+extern "C" int dexr_solve_jacobian(const dexr_robot_t* robot, const dexr_params_t* params, const dexr_jacobian_t* io,
+                                   int64_t num_frames, void* cuda_stream) {
+  if (!robot || !params || !io) return fail(DEXR_E_INVALID, "dexr_solve_jacobian: null argument");
+  if (num_frames < 0) return fail(DEXR_E_INVALID, "num_frames < 0");
+  if (const char* msg = jacobian_io_error(robot->host, *io, *params)) return fail(DEXR_E_INVALID, "%s", msg);
+  if (int e = check_loss_params(params)) return e;
+  if (num_frames == 0) return 0;
+  DEVICE_SCOPE(robot->device);
+  dexr_robot* r = const_cast<dexr_robot*>(robot);
+  cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
+  return eval_lanes(r->host) == 16 ? launch_jacobian<16>(r, params, io, num_frames, stream)
+                                   : launch_jacobian<32>(r, params, io, num_frames, stream);
 }
 
 extern "C" int dexr_solve_frames_multi(const dexr_group_t* groups, int32_t num_groups, void* cuda_stream) {

@@ -1778,7 +1778,7 @@ __device__ __forceinline__ void vjp_column(const Solver<G, 0>& sv, int k, float&
   }
 }
 
-// What vjp_core hands back to its driver, per lane: v (H_ff^-1 gbar_f on this lane's variable, 0 elsewhere), the fixed-joint
+// What vjp_tail hands back to its driver, per lane: v (H_ff^-1 gbar_f on this lane's variable, 0 elsewhere), the fixed-joint
 // term H_q[c, :] . M v of a fixed lane (its cotangent is -qbar), and the frame's finite / not-positive-definite verdicts
 // (group-uniform).  The keypoint cotangents are in the scratch's kKp accumulator.
 struct VjpLane {
@@ -1786,14 +1786,23 @@ struct VjpLane {
   bool finite, bad;
 };
 
-// The per-frame core of the implicit-function VJP, shared by vjp_frame (dexr_solve_vjp) and vjp_stream
-// (dexr_solve_sequences_vjp): the point x, the anchor x0 and the cotangent gbar of this lane's variable come from the driver,
-// with norm_delta `nd` (0: no regulariser) and the frame's DexPilot flags `proj` (read into the scratch; nullptr = all 0).
-// Writes the ref_value cotangents to `grad_ref` ([m,3] of the frame, or nullptr) itself; everything else goes back to the
-// driver.  The caller's flags are never written.
+// What vjp_front leaves for vjp_tail besides the scratch (H_q in kH, the factor in kA, the flags in kFlags): whether this
+// lane's variable is free, and the frame's finite / not-positive-definite verdicts (group-uniform).
+struct VjpFront {
+  bool free_, finite, bad;
+};
+
+// The implicit-function VJP of one frame is vjp_front once, then vjp_tail once per cotangent: vjp_frame (dexr_solve_vjp) and
+// vjp_stream (dexr_solve_sequences_vjp) run one tail, jacobian_frame (dexr_solve_jacobian) one per free variable.
+//
+// The per-frame front: the point x, the anchor x0 of this lane's variable come from the driver, with norm_delta `nd`
+// (0: no regulariser) and the frame's DexPilot flags `proj` (read into the scratch; nullptr = all 0); `gbar` only takes
+// part in the finiteness verdict.  Prepares the targets on the private flag copy, runs FK, builds the gradient, the active
+// set and the exact H_q, folds the mimic joints, freezes the active rows and factorises the free block in place in kA.  The
+// caller's flags are never written.
 template <int G>
-__device__ __forceinline__ VjpLane vjp_core(Solver<G, 0>& sv, const FrameInputs& in_, const Dims& dm, float x, float x0,
-                                            float gbar, float nd, const uint8_t* proj, float* grad_ref, bool active) {
+__device__ __forceinline__ VjpFront vjp_front(Solver<G, 0>& sv, const FrameInputs& in_, const Dims& dm, float x, float x0,
+                                              float gbar, float nd, const uint8_t* proj, bool active) {
   using VS = VjpScratch<G>;
   constexpr int NP = G;
   const SharedTable& st = Solver<G, 0>::ST();
@@ -1801,8 +1810,6 @@ __device__ __forceinline__ VjpLane vjp_core(Solver<G, 0>& sv, const FrameInputs&
   const bool isvar = sv.var >= 0;
   float* const hq = sv.scf() + VS::kH;
   float* const A = sv.scf() + VS::kA;
-  float* const mvs = sv.scf() + VS::kMv;
-  float* const kpacc = sv.scf() + VS::kKp;
   uint8_t* const flags = reinterpret_cast<uint8_t*>(sv.scf() + VS::kFlags);
 
   // ---- targets (flags on the private copy), FK at x
@@ -1810,7 +1817,6 @@ __device__ __forceinline__ VjpLane vjp_core(Solver<G, 0>& sv, const FrameInputs&
   sv.qfix = (active && fixedi >= 0) ? in_.fixed[fixedi] : 0.f;
   sv.x = x;
   if (l < dm.len_proj) flags[l] = (active && proj) ? proj[l] : (uint8_t)0;
-  for (int e = l; e < 64; e += G) kpacc[e] = 0.f;
   __syncwarp();
   FrameInputs in = in_;
   in.projected = dm.len_proj > 0 ? flags : nullptr;
@@ -1950,6 +1956,34 @@ __device__ __forceinline__ VjpLane vjp_core(Solver<G, 0>& sv, const FrameInputs&
     }
   }
   __syncwarp();
+  return VjpFront{free_, finite, bad};
+}
+
+// The per-cotangent tail, after vjp_front on the same frame (`fr` its result, `in_` the frame inputs it was given):
+// gbar = dl/dx of this lane's variable.  Solves H_ff v = gbar_f with the factor in kA, maps v to joint space (M v), runs the
+// target pass -- the ref_value cotangents go to `grad_ref` ([m,3] of the frame, or nullptr), the keypoint ones to the kKp
+// accumulator, which it clears first -- and forms the fixed-joint term; everything but grad_ref goes back to the driver.
+// Reads the scratch the front left and writes only kMv and kKp, so it can run any number of times after one front.
+template <int G>
+__device__ __forceinline__ VjpLane vjp_tail(Solver<G, 0>& sv, const FrameInputs& in_, const Dims& dm, const VjpFront& fr,
+                                            float gbar, float* grad_ref, bool active) {
+  using VS = VjpScratch<G>;
+  constexpr int NP = G;
+  const SharedTable& st = Solver<G, 0>::ST();
+  const int l = sv.l, dof = dm.dof, m = dm.n_res;
+  const bool isvar = sv.var >= 0;
+  const bool free_ = fr.free_, finite = fr.finite, bad = fr.bad;
+  const float* const hq = sv.scf() + VS::kH;
+  const float* const A = sv.scf() + VS::kA;
+  float* const mvs = sv.scf() + VS::kMv;
+  float* const kpacc = sv.scf() + VS::kKp;
+  const uint8_t* const flags = reinterpret_cast<const uint8_t*>(sv.scf() + VS::kFlags);
+  const FrameInputs& in = in_;
+  const int fixedi = st.fixed_index[l];
+  const float beta = sv.prm.huber_delta, inv_beta = sv.inv_beta;
+  const bool pos_loss = dm.loss == DEXR_LOSS_POSITION;
+  for (int e = l; e < 64; e += G) kpacc[e] = 0.f;  // (the driver reads its entries of the previous tail on the same lane)
+
   // v = A^-1 gbar (forward, then back substitution; frozen rows are identity rows with a zero right-hand side)
   float y = free_ ? gbar : 0.f;
   for (int k = 0; k < dof; ++k) {
@@ -2045,8 +2079,8 @@ __device__ __forceinline__ void vjp_frame(Solver<G, 0>& sv, const FrameInputs& i
     gbar = io.grad_qpos[f * dm.n_var + sv.var];
   }
   const float nd = io.last_qpos ? sv.prm.norm_delta : 0.f;  // no anchor: no regulariser
-  const VjpLane r = vjp_core(sv, in, dm, x, x0, gbar, nd, io.projected ? io.projected + f * dm.len_proj : nullptr,
-                             io.grad_ref_value ? io.grad_ref_value + f * dm.n_res * 3 : nullptr, active);
+  const VjpFront fr = vjp_front(sv, in, dm, x, x0, gbar, nd, io.projected ? io.projected + f * dm.len_proj : nullptr, active);
+  const VjpLane r = vjp_tail(sv, in, dm, fr, gbar, io.grad_ref_value ? io.grad_ref_value + f * dm.n_res * 3 : nullptr, active);
   const int fixedi = Solver<G, 0>::ST().fixed_index[l];
   const bool by_kp = in.kp != nullptr;
   const float* const kpacc = sv.scf() + VjpScratch<G>::kKp;
@@ -2059,6 +2093,71 @@ __device__ __forceinline__ void vjp_frame(Solver<G, 0>& sv, const FrameInputs& i
       for (int e = l; e < 3 * DEXR_NUM_KEYPOINTS; e += G) io.grad_keypoints[f * 3 * DEXR_NUM_KEYPOINTS + e] = out(kpacc[e]);
     if (l == 0 && io.status_out) io.status_out[f] = !r.finite ? DEXR_STATUS_NONFINITE : (r.bad ? DEXR_STATUS_NOT_PD : 0);
   }
+  __syncwarp();  // the group's next frame rewrites the scratch this one read
+}
+
+// ------------------------------------------------------------------------------------------------
+// per-frame Jacobians of the solve (dexr_solve_jacobian): one front, then one tail per free variable
+// ------------------------------------------------------------------------------------------------
+// The argument checks of dexr_solve_jacobian that read the robot's table: nullptr, or what is wrong.  Host code shared by
+// the library and the host emulation, as vjp_io_error.
+inline const char* jacobian_io_error(const dexr_table_t& t, const dexr_jacobian_t& io, const dexr_params_t& prm) {
+  if (!io.qpos) return "qpos is required";
+  if ((io.keypoints != nullptr) == (io.ref_value != nullptr)) return "exactly one of keypoints / ref_value must be given";
+  if (prm.preprocess != 0) return "raw-landmark pre-processing is not differentiated: params.preprocess must be 0";
+  if (t.n_fixed > 0 && !io.fixed_qpos) return "the robot has fixed joints but fixed_qpos is NULL";
+  if (io.jac_keypoints && !io.keypoints) return "jac_keypoints needs the keypoints form";
+  if (io.jac_ref_value && !io.ref_value) return "jac_ref_value needs the ref_value form";
+  if (io.jac_last_qpos && !io.last_qpos) return "jac_last_qpos needs last_qpos";
+  return nullptr;
+}
+
+// One frame of dexr_solve_jacobian (see dexr.h): vjp_front once, then for every variable i the row of cotangent e_i --
+// vjp_tail with gbar = e_i where i is free, a zero row where it is active.  The warp's groups hold different frames but run
+// the tail's collectives together: a row runs the tail when it is free in some group's frame, and a group whose own row i
+// is active (or whose frame is bad) writes zeros (NaN for a non-finite frame) from it.  Row i of the frame is written from
+// kpacc (keypoints), by the tail itself (ref_value), -qbar (fixed joints) and 2 norm_delta v (anchor).
+template <int G>
+__device__ __forceinline__ void jacobian_frame(Solver<G, 0>& sv, const FrameInputs& in, const dexr_jacobian_t& io,
+                                               const Dims& dm, long long f, bool active) {
+  const int l = sv.l, lane = sv.lane, n = dm.n_var;
+  const bool isvar = sv.var >= 0;
+  float x = 0.f, x0 = 0.f;
+  if (active && isvar) {
+    x = io.qpos[f * n + sv.var];
+    x0 = io.last_qpos ? io.last_qpos[f * n + sv.var] : x;
+  }
+  const float nd = io.last_qpos ? sv.prm.norm_delta : 0.f;  // no anchor: no regulariser
+  const VjpFront fr = vjp_front(sv, in, dm, x, x0, 0.f, nd, io.projected ? io.projected + f * dm.len_proj : nullptr, active);
+  const int fixedi = Solver<G, 0>::ST().fixed_index[l];
+  const bool by_kp = in.kp != nullptr;
+  const float* const kpacc = sv.scf() + VjpScratch<G>::kKp;
+  const float nan = __int_as_float(0x7fc00000);
+  // a zero row for an active variable or a not-positive-definite frame, NaN for a frame with a non-finite input
+  const float zero = fr.finite ? 0.f : nan;
+  const bool good = active && fr.finite && !fr.bad;
+  for (int i = 0; i < n; ++i) {
+    const long long row = f * n + i;
+    // row i of this group's frame needs the tail when variable i is free there; the warp runs it when some group needs it
+    const unsigned need = __ballot_sync(0xffffffffu, good && fr.free_ && sv.var == i);
+    const bool here = G == 32 ? need != 0u : ((need >> (lane & ~(G - 1))) & ((1u << (G & 31)) - 1u)) != 0u;
+    float v = 0.f, qbar = 0.f;
+    if (need != 0u) {  // (warp-uniform)
+      const VjpLane r = vjp_tail(sv, in, dm, fr, sv.var == i ? 1.0f : 0.f,
+                                 here && io.jac_ref_value ? io.jac_ref_value + row * dm.n_res * 3 : nullptr, active);
+      v = r.v;
+      qbar = r.qbar;
+    }
+    if (active) {
+      if (isvar && io.jac_last_qpos) io.jac_last_qpos[row * n + sv.var] = here ? 2.0f * nd * v : zero;
+      if (fixedi >= 0 && io.jac_fixed_qpos) io.jac_fixed_qpos[row * dm.n_fixed + fixedi] = here ? -qbar : zero;
+      if (by_kp && io.jac_keypoints)
+        for (int e = l; e < 3 * DEXR_NUM_KEYPOINTS; e += G) io.jac_keypoints[row * 3 * DEXR_NUM_KEYPOINTS + e] = here ? kpacc[e] : zero;
+      if (!here && !by_kp && io.jac_ref_value && l < 3)
+        for (int k = 0; k < dm.n_res; ++k) io.jac_ref_value[row * dm.n_res * 3 + k * 3 + l] = zero;
+    }
+  }
+  if (active && l == 0 && io.status_out) io.status_out[f] = !fr.finite ? DEXR_STATUS_NONFINITE : (fr.bad ? DEXR_STATUS_NOT_PD : 0);
   __syncwarp();  // the group's next frame rewrites the scratch this one read
 }
 
@@ -2081,7 +2180,7 @@ inline const char* seq_vjp_io_error(const dexr_table_t& t, const dexr_sequences_
 
 // One stream s of S, walked from its last frame to its first (dexr.h, dexr_solve_sequences_vjp): gy (the filter's cotangent,
 // lane = joint) and c (the anchor cotangent flowing to the previous solution, lane = variable) stay in registers between
-// frames; each frame runs vjp_core at (x_t, clip(x_{t-1})) with gbar = M^T gq + c.  A group that is not `active` walks
+// frames; each frame runs vjp_front and vjp_tail at (x_t, clip(x_{t-1})) with gbar = M^T gq + c.  A group that is not `active` walks
 // stream S - 1 and writes nothing.  `dm`, S and steps are the kernel argument's, as in solve_stream.
 template <int G>
 __device__ __forceinline__ void vjp_stream(Solver<G, 0>& sv, const dexr_sequences_vjp_t& io, const Dims& dm, const long long& S,
@@ -2134,8 +2233,8 @@ __device__ __forceinline__ void vjp_stream(Solver<G, 0>& sv, const dexr_sequence
     in.fixed = dm.n_fixed > 0 ? io.fixed_qpos + fr * dm.n_fixed : nullptr;
     in.last = nullptr;
     in.projected = nullptr;
-    const VjpLane r = vjp_core(sv, in, dm, x, a, gbar, nd, io.projected ? io.projected + fr * dm.len_proj : nullptr,
-                               nullptr, active);
+    const VjpFront vf = vjp_front(sv, in, dm, x, a, gbar, nd, io.projected ? io.projected + fr * dm.len_proj : nullptr, active);
+    const VjpLane r = vjp_tail(sv, in, dm, vf, gbar, nullptr, active);
     // outputs: NaN for a frame with a non-finite input (and, through c, for every earlier frame of the stream); v = 0 for
     // one whose free Hessian is not positive definite
     auto out = [&](float val) { return !r.finite ? __int_as_float(0x7fc00000) : val; };

@@ -487,6 +487,51 @@ class Optimizer:
         N.check(eng.lib.dexr_solve_vjp(eng.handle, C.byref(p), C.byref(io), B, C.c_void_p(s.cuda_stream)), "dexr_solve_vjp")
         return g_tgt, g_fixed, g_last
 
+    def retarget_batch_jacobian(self, qpos, ref_value=None, fixed_qpos=None, last_qpos=None, *, keypoints=None,
+                                projected=None, jac_keypoints_out=None, jac_ref_value_out=None, jac_fixed_qpos_out=None,
+                                jac_last_qpos_out=None, status_out=None, stream=None):
+        """Per-frame Jacobians dqpos/dtheta of the solve at B points, one launch (`dexr_solve_jacobian`).  Arguments as for
+        `retarget_batch_vjp` without the cotangent.  Row i of every block is what `retarget_batch_vjp` returns for the
+        cotangent e_i (the unit vector of variable i): the same point, anchor, flags, active set and exact Hessian, factorised
+        once per frame.  Rows of active variables are zero; the anchor block is 2 norm_delta H_ff^-1.
+        Returns (jac_targets, jac_fixed_qpos, jac_last_qpos), CUDA tensors: jac_targets [B,opt_dof,21,3] for keypoints or
+        [B,opt_dof,m,3] for ref_value, jac_fixed_qpos [B,opt_dof,n_fixed] (None without fixed joints), jac_last_qpos
+        [B,opt_dof,opt_dof] (None without last_qpos).  `status_out` [B] int32 as for `retarget_batch_vjp` (STATUS_NOT_PD
+        frames get zeros, STATUS_NONFINITE frames NaN).  Nothing is synchronised."""
+        import torch
+
+        eng = self.engine()
+        dev = torch.device("cuda", eng.device)
+        chk = _tensor_check(dev)
+        B = qpos.shape[0]
+        n, nf = self.opt_dof, len(self.idx_pin2fixed)
+        io = N.DexrJacobian()
+        io.qpos = chk(qpos, (B, n), torch.float32, "qpos")
+        self._batch_targets(io, chk, B, ref_value, keypoints, fixed_qpos, last_qpos=last_qpos)
+        if projected is not None:
+            io.projected = chk(projected, (B, self._objective_spec().len_proj), torch.uint8, "projected")
+
+        def out(t, shape, name):
+            t = torch.empty(shape, dtype=torch.float32, device=dev) if t is None else t
+            return t, chk(t, shape, torch.float32, name)
+
+        if keypoints is not None:
+            j_tgt, io.jac_keypoints = out(jac_keypoints_out, (B, n, N.NUM_KEYPOINTS, 3), "jac_keypoints_out")
+        else:
+            j_tgt, io.jac_ref_value = out(jac_ref_value_out, (B, n, self.num_residuals, 3), "jac_ref_value_out")
+        j_fixed = j_last = None
+        if nf:
+            j_fixed, io.jac_fixed_qpos = out(jac_fixed_qpos_out, (B, n, nf), "jac_fixed_qpos_out")
+        if last_qpos is not None:
+            j_last, io.jac_last_qpos = out(jac_last_qpos_out, (B, n, n), "jac_last_qpos_out")
+        if status_out is not None:
+            io.status_out = chk(status_out, (B,), torch.int32, "status_out")
+        p = self.params()
+        s = stream if stream is not None else torch.cuda.current_stream(dev)
+        N.check(eng.lib.dexr_solve_jacobian(eng.handle, C.byref(p), C.byref(io), B, C.c_void_p(s.cuda_stream)),
+                "dexr_solve_jacobian")
+        return j_tgt, j_fixed, j_last
+
     def _objective_flags(self):
         """Hysteresis state an objective closure starts from (DexPilot only)."""
         return None

@@ -360,6 +360,35 @@ size_t dexr_sequences_vjp_sizeof(void);
 int dexr_solve_sequences_vjp(const dexr_robot_t* robot, const dexr_params_t* params, const dexr_sequences_vjp_t* io,
                              int64_t num_streams, int64_t num_steps, void* cuda_stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Per-frame Jacobians of the solve: J = dx/dtheta of frame f's solution x with respect to its inputs theta (the keypoints
+ * or ref_value, the fixed joints and the anchor last_qpos), in one launch for all frames.  Row i of every block is exactly
+ * what dexr_solve_vjp writes for the same frame with grad_qpos = e_i (the unit cotangent of variable i), so everything is
+ * the VJP's: the point, the anchor, the read-only DexPilot flags, the solver's active-set rule, the exact Hessian, the
+ * one-sided derivative at a Huber zone or flag switch, and the status bits.  Hence: the rows of active variables are zero;
+ * the anchor block is 2 norm_delta H_ff^-1, with zero rows and columns for the active variables; a DEXR_STATUS_NOT_PD frame
+ * gets all zeros and a frame with a non-finite input gets NaN and DEXR_STATUS_NONFINITE (no other frame changes).  The
+ * Hessian is factorised once per frame and every free variable's row reuses the factor.  Uncertainty propagation is
+ * Sigma_q = J Sigma_theta J^T.  params.preprocess must be 0 (raw landmarks are not differentiated).  Asynchronous on
+ * `cuda_stream`, allocates nothing; num_frames == 0 does nothing.  All pointers are DEVICE pointers.
+ * ------------------------------------------------------------------------------------------- */
+typedef struct dexr_jacobian {
+  const float* keypoints;   /* [B,21,3] or NULL  } exactly one of the two                                            */
+  const float* ref_value;   /* [B,m,3]  or NULL  }                                                                   */
+  const float* fixed_qpos;  /* [B,n_fixed] or NULL when n_fixed == 0                                                 */
+  const float* qpos;        /* [B,n_var] the point x                                                                 */
+  const float* last_qpos;   /* [B,n_var] anchor of the norm_delta term, or NULL: no regulariser                      */
+  const uint8_t* projected; /* [B,len_proj] DexPilot flags, read only; NULL as in dexr_vjp_t                         */
+  float* jac_keypoints;     /* [B,n_var,21,3] or NULL (keypoints form only; all 63 columns written)                  */
+  float* jac_ref_value;     /* [B,n_var,m,3]  or NULL (ref_value form only)                                          */
+  float* jac_fixed_qpos;    /* [B,n_var,n_fixed] or NULL                                                             */
+  float* jac_last_qpos;     /* [B,n_var,n_var] or NULL (needs last_qpos)                                             */
+  int32_t* status_out;      /* [B] or NULL: 0, DEXR_STATUS_NONFINITE or DEXR_STATUS_NOT_PD                           */
+} dexr_jacobian_t;
+size_t dexr_jacobian_sizeof(void);
+int dexr_solve_jacobian(const dexr_robot_t* robot, const dexr_params_t* params, const dexr_jacobian_t* io,
+                        int64_t num_frames, void* cuda_stream);
+
 #ifdef __cplusplus
 }
 #endif
