@@ -137,7 +137,7 @@ EXPORTS = [
     "dexr_solve_frames", "dexr_solve_frames_multi", "dexr_solve_sequences", "dexr_solve_frames_host", "dexr_get_launch_info",
     "dexr_preprocess_keypoints", "dexr_eval_sizeof", "dexr_eval_objective", "dexr_vjp_sizeof", "dexr_solve_vjp",
     "dexr_sequences_tape_sizeof", "dexr_solve_sequences_tape", "dexr_sequences_vjp_sizeof", "dexr_solve_sequences_vjp",
-    "dexr_jacobian_sizeof", "dexr_solve_jacobian",
+    "dexr_jacobian_sizeof", "dexr_solve_jacobian", "dexr_solve_sequences_packed", "dexr_solve_sequences_packed_vjp",
 ]
 
 _LIB = None
@@ -231,6 +231,15 @@ def load():
                                             C.c_void_p]
     elif not os.environ.get("DEXR_LIBRARY"):
         raise DexrError(f"{path} does not export dexr_jacobian_sizeof: rebuild it (python -m dex_retargeting_b200.build --force)")
+    if hasattr(lib, "dexr_solve_sequences_packed"):
+        lib.dexr_solve_sequences_packed.argtypes = [C.c_void_p, C.POINTER(DexrParams), C.POINTER(DexrSequences),
+                                                    C.POINTER(DexrSequencesTape), C.c_void_p, C.c_int64, C.c_int64,
+                                                    C.c_void_p]
+        lib.dexr_solve_sequences_packed_vjp.argtypes = [C.c_void_p, C.POINTER(DexrParams), C.POINTER(DexrSequencesVjp),
+                                                        C.c_void_p, C.c_int64, C.c_int64, C.c_void_p]
+    elif not os.environ.get("DEXR_LIBRARY"):
+        raise DexrError(f"{path} does not export dexr_solve_sequences_packed: rebuild it "
+                        "(python -m dex_retargeting_b200.build --force)")
     # (an older A/B library named by DEXR_LIBRARY reads a prefix of the buffer structs -- fields are only ever appended -- so
     # the single-robot entry points still work with it; dexr_solve_frames_multi, whose groups embed the struct, does not)
     _LIB = lib

@@ -274,6 +274,38 @@ __global__ void __launch_bounds__(NW * 32, 1) dexr_sequences_tape_kernel(const S
   }
 }
 
+// dexr_solve_sequences_packed: dexr_sequences_kernel's launch shape and stream slots, stream s with its frames at
+// pk.offsets (solve_packed_stream); REC records the tape.  a.steps is not read.
+template <int G, int BW, int NW, bool REC>
+__global__ void __launch_bounds__(NW * 32, 1) dexr_packed_sequences_kernel(const SeqArgs a, const PackedLayout pk,
+                                                                           const dexr_sequences_tape_t tape) {
+  unsigned char* const smem = dsmem;
+  SharedTable* st = reinterpret_cast<SharedTable*>(smem);
+  load_shared_table(*st, a.table, pass_slot_width<BW>());
+  __syncthreads();
+
+  constexpr int GPW = 32 / G;
+  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
+  const int lane = threadIdx.x & 31;
+  const int gid = warp * GPW + (lane / G);
+  const int slots_per_cta = NW * a.spw;
+  const uint32_t scratch_off = (uint32_t)(a.scratch_off + gid * Scratch<G, BW>::kStreamFloats * 4);
+  float* kpbuf = reinterpret_cast<float*>(smem + scratch_off) + Scratch<G, BW>::kFloats;
+  const int slot = a.spw == GPW ? gid : warp;
+  const bool first = (lane / G) == 0;
+  const bool owner = a.spw == GPW || first;
+  const bool works = owner || a.duo;
+  Solver<G, BW> sv;
+  sv.init(a.table, a.dm, scratch_off, a.prm, lane);
+  if (G == 16 && a.duo) sv.duo = lane / G;
+  const bool use_filter = a.prm.lp_alpha >= 0.f && a.prm.lp_alpha <= 1.f;
+
+  for (long long base = 0; base < a.S; base += (long long)gridDim.x * slots_per_cta) {
+    const PackedStream ps = packed_stream(pk, base + (long long)slot * gridDim.x + blockIdx.x);
+    solve_packed_stream<G, BW, REC>(sv, a.io, a.dm, a.prm, ps, works, owner, kpbuf, use_filter, tape.qpos, tape.projected);
+  }
+}
+
 // ------------------------------------------------------------------------------------------------
 // objective evaluation: one frame per group of G lanes, groups striding over the batch
 // ------------------------------------------------------------------------------------------------
@@ -429,6 +461,28 @@ __global__ void __launch_bounds__(kEvalWarps * 32, G == 16 ? 2 : 1) dexr_seq_vjp
     if (base + (long long)first_slot * gridDim.x + blockIdx.x >= a.S) continue;
     const long long s = base + (long long)slot * gridDim.x + blockIdx.x;
     vjp_stream(sv, a.io, a.dm, a.S, a.steps, s, owner && s < a.S, use_filter);
+  }
+}
+
+// dexr_solve_sequences_packed_vjp: dexr_seq_vjp_kernel's launch shape and stream slots over the packed streams
+// (vjp_packed_stream; a warp without a stream has no steps and moves on).  a.steps is not read.
+template <int G>
+__global__ void __launch_bounds__(kEvalWarps * 32, G == 16 ? 2 : 1) dexr_packed_seq_vjp_kernel(const SeqVjpArgs a,
+                                                                                               const PackedLayout pk) {
+  load_shared_table(*reinterpret_cast<SharedTable*>(dsmem), a.table);
+  __syncthreads();
+  constexpr int GPW = 32 / G;
+  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
+  const int lane = threadIdx.x & 31;
+  const int gid = warp * GPW + lane / G;
+  Solver<G, 0> sv;
+  sv.init(a.table, a.dm, (uint32_t)(a.scratch_off + gid * VjpScratch<G>::kFloats * 4), a.prm, lane);
+  const int slot = a.spw == GPW ? gid : warp;
+  const bool owner = a.spw == GPW || lane < G;
+  const bool use_filter = a.prm.lp_alpha >= 0.f && a.prm.lp_alpha <= 1.f;
+  for (long long base = 0; base < a.S; base += (long long)gridDim.x * kEvalWarps * a.spw) {
+    const PackedStream ps = packed_stream(pk, base + (long long)slot * gridDim.x + blockIdx.x);
+    vjp_packed_stream(sv, a.io, a.dm, ps, owner, use_filter);
   }
 }
 
@@ -1200,6 +1254,24 @@ extern "C" int dexr_solve_frames(const dexr_robot_t* robot, const dexr_params_t*
   return launch_frames_kind(r, params, io, num_frames, stream);
 }
 
+// Launch shape of the sequences kernels for S streams: sets a.spw and a.duo, returns the grid.
+// A stream is serial in time and latency bound, so streams are spread over as many warps and SMs as there are: while one
+// warp per stream fits into one wave of CTAs (S <= SMs x warps per CTA), a warp carries ONE stream (the second group of a
+// 16-lane solver idles); beyond that two 16-lane streams share a warp.  One CTA per SM, two when streams are plentiful.
+template <int G>
+static int sequences_shape(const dexr_robot* r, long long S, SeqArgs& a) {
+  constexpr int GPW = 32 / G;
+  const long long warps_one_wave = (long long)r->num_sms * kSeqNW;
+  a.spw = (GPW > 1 && S > warps_one_wave) ? GPW : 1;
+  static const int spw_env = [] { const char* e = getenv("DEXR_SEQ_PAIR"); return e ? atoi(e) : -1; }();  // A/B: 1 = always pair
+  if (spw_env == 1) a.spw = GPW;
+  const char* duo_env = getenv("DEXR_SEQ_DUO");  // 0 = off (read per call: tests compare the two modes in one process)
+  a.duo = (G == 16 && a.spw == 1 && !(duo_env && atoi(duo_env) == 0)) ? 1 : 0;
+  const long long per_cta = (long long)kSeqNW * a.spw;
+  const long long ctas = std::max<long long>(1, (S + a.spw - 1) / a.spw);  // at least one warp's worth of streams per CTA
+  return (int)std::min<long long>(ctas, (long long)r->num_sms * (S >= (long long)r->num_sms * per_cta * 2 ? 2 : 1));
+}
+
 template <int G, int BW>
 static int launch_sequences(dexr_robot* r, const dexr_params_t* prm, const dexr_sequences_t* io, long long S, int steps,
                             cudaStream_t stream, const dexr_sequences_tape_t* tape = nullptr) {
@@ -1219,20 +1291,35 @@ static int launch_sequences(dexr_robot* r, const dexr_params_t* prm, const dexr_
   auto kern_tape = dexr_sequences_tape_kernel<G, BW, kSeqNW>;
   if (tape) CUDA_TRY(cudaFuncSetAttribute(kern_tape, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
   else CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  // A stream is serial in time and latency bound, so streams are spread over as many warps and SMs as there are: while one
-  // warp per stream fits into one wave of CTAs (S <= SMs x warps per CTA), a warp carries ONE stream (the second group of a
-  // 16-lane solver idles); beyond that two 16-lane streams share a warp.  One CTA per SM, two when streams are plentiful.
-  const long long warps_one_wave = (long long)r->num_sms * kSeqNW;
-  a.spw = (GPW > 1 && S > warps_one_wave) ? GPW : 1;
-  static const int spw_env = [] { const char* e = getenv("DEXR_SEQ_PAIR"); return e ? atoi(e) : -1; }();  // A/B: 1 = always pair
-  if (spw_env == 1) a.spw = GPW;
-  const char* duo_env = getenv("DEXR_SEQ_DUO");  // 0 = off (read per call: tests compare the two modes in one process)
-  a.duo = (G == 16 && a.spw == 1 && !(duo_env && atoi(duo_env) == 0)) ? 1 : 0;
-  const long long per_cta = (long long)kSeqNW * a.spw;
-  const long long ctas = std::max<long long>(1, (S + a.spw - 1) / a.spw);  // at least one warp's worth of streams per CTA
-  int grid = (int)std::min<long long>(ctas, (long long)r->num_sms * (S >= (long long)r->num_sms * per_cta * 2 ? 2 : 1));
+  const int grid = sequences_shape<G>(r, S, a);
   if (tape) kern_tape<<<grid, kSeqNW * 32, smem, stream>>>(a, *tape);
   else kern<<<grid, kSeqNW * 32, smem, stream>>>(a);
+  CUDA_TRY(cudaGetLastError());
+  {
+    std::lock_guard<std::mutex> lk(r->info_mu);
+    r->last = dexr_launch_info_t{grid, kSeqNW * 32, smem, 0, G, kSeqNW, r->last.kernels_launched + 1};
+  }
+  return 0;
+}
+
+// dexr_solve_sequences_packed: launch_sequences for S packed streams (same shape, spw, duo and grid).
+template <int G, int BW>
+static int launch_packed_sequences(dexr_robot* r, const dexr_params_t* prm, const dexr_sequences_t* io, const PackedLayout& pk,
+                                   cudaStream_t stream, const dexr_sequences_tape_t* tape) {
+  SeqArgs a{};
+  a.table = r->table_dev;
+  a.prm = sequence_params(*prm);
+  a.io = *io;
+  a.S = pk.S;
+  a.dm = make_dims(r->host);
+  a.scratch_off = round_up((int)sizeof(SharedTable), 16);
+  const int smem = a.scratch_off + kSeqNW * (32 / G) * Scratch<G, BW>::kStreamFloats * 4;
+  auto kern = dexr_packed_sequences_kernel<G, BW, kSeqNW, false>;
+  auto kern_tape = dexr_packed_sequences_kernel<G, BW, kSeqNW, true>;
+  CUDA_TRY(cudaFuncSetAttribute(tape ? kern_tape : kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  const int grid = sequences_shape<G>(r, pk.S, a);
+  if (tape) kern_tape<<<grid, kSeqNW * 32, smem, stream>>>(a, pk, *tape);
+  else kern<<<grid, kSeqNW * 32, smem, stream>>>(a, pk, dexr_sequences_tape_t{nullptr, nullptr});
   CUDA_TRY(cudaGetLastError());
   {
     std::lock_guard<std::mutex> lk(r->info_mu);
@@ -1326,6 +1413,70 @@ extern "C" int dexr_solve_sequences_vjp(const dexr_robot_t* robot, const dexr_pa
   cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
   return eval_lanes(r->host) == 16 ? launch_seq_vjp<16>(r, params, io, num_streams, (int)num_steps, stream)
                                    : launch_seq_vjp<32>(r, params, io, num_streams, (int)num_steps, stream);
+}
+
+extern "C" int dexr_solve_sequences_packed(const dexr_robot_t* robot, const dexr_params_t* params, const dexr_sequences_t* io,
+                                           const dexr_sequences_tape_t* tape, const int64_t* offsets, int64_t num_streams, int64_t num_frames, void* cuda_stream) {
+  if (!robot || !params || !io) return fail(DEXR_E_INVALID, "dexr_solve_sequences_packed: null argument");
+  if (const char* msg = packed_io_error(robot->host, *io, tape, *params, offsets, num_streams, num_frames))
+    return fail(DEXR_E_INVALID, "%s", msg);
+  if (num_streams == 0 || num_frames == 0) return 0;
+  if (int e = check_params(params)) return e;
+  DEVICE_SCOPE(robot->device);
+  dexr_robot* r = const_cast<dexr_robot*>(robot);
+  cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
+  const PackedLayout pk{offsets, num_streams, num_frames};
+  dexr_sequences_tape_t tp{nullptr, nullptr};
+  if (tape) tp = dexr_sequences_tape_t{tape->qpos, robot->host.loss == DEXR_LOSS_DEXPILOT ? tape->projected : nullptr};
+  return with_solver(solver_kind(r->host, arrow_enabled()), [&](auto s) {
+    return launch_packed_sequences<decltype(s)::G, decltype(s)::BW>(r, params, io, pk, stream, tape ? &tp : nullptr);
+  });
+}
+
+// dexr_solve_sequences_packed_vjp: launch_seq_vjp's shape (and A/B switches) for S packed streams.
+template <int G>
+static int launch_packed_seq_vjp(dexr_robot* r, const dexr_params_t* prm, const dexr_sequences_vjp_t* io, const PackedLayout& pk,
+                                 cudaStream_t stream) {
+  SeqVjpArgs a{};
+  a.table = r->table_dev;
+  a.prm = sequence_params(*prm);
+  a.io = *io;
+  a.S = pk.S;
+  a.dm = make_dims(r->host);
+  a.scratch_off = round_up((int)sizeof(SharedTable), 16);
+  constexpr int GPW = 32 / G;
+  a.spw = GPW;
+  if (const char* e = getenv("DEXR_SEQ_VJP_SPW"))
+    if (atoi(e) == 1) a.spw = 1;
+  const int smem = a.scratch_off + kEvalWarps * GPW * VjpScratch<G>::kFloats * 4;
+  auto kern = dexr_packed_seq_vjp_kernel<G>;
+  CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  int per_sm = 1;
+  if (int e = eval_ctas_per_sm(kern, smem, &per_sm)) return e;
+  const long long ctas = (pk.S + a.spw - 1) / a.spw;
+  const int grid = (int)std::min<long long>(ctas, (long long)r->num_sms * per_sm);
+  kern<<<grid, kEvalWarps * 32, smem, stream>>>(a, pk);
+  CUDA_TRY(cudaGetLastError());
+  {
+    std::lock_guard<std::mutex> lk(r->info_mu);
+    r->last = dexr_launch_info_t{grid, kEvalWarps * 32, smem, 0, G, kEvalWarps, r->last.kernels_launched + 1};
+  }
+  return 0;
+}
+
+extern "C" int dexr_solve_sequences_packed_vjp(const dexr_robot_t* robot, const dexr_params_t* params,
+                                               const dexr_sequences_vjp_t* io, const int64_t* offsets, int64_t num_streams, int64_t num_frames, void* cuda_stream) {
+  if (!robot || !params || !io) return fail(DEXR_E_INVALID, "dexr_solve_sequences_packed_vjp: null argument");
+  if (const char* msg = packed_io_error(robot->host, *io, *params, offsets, num_streams, num_frames))
+    return fail(DEXR_E_INVALID, "%s", msg);
+  if (int e = check_loss_params(params)) return e;
+  if (num_streams == 0 || num_frames == 0) return 0;
+  DEVICE_SCOPE(robot->device);
+  dexr_robot* r = const_cast<dexr_robot*>(robot);
+  cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
+  const PackedLayout pk{offsets, num_streams, num_frames};
+  return eval_lanes(r->host) == 16 ? launch_packed_seq_vjp<16>(r, params, io, pk, stream)
+                                   : launch_packed_seq_vjp<32>(r, params, io, pk, stream);
 }
 
 extern "C" {

@@ -2257,4 +2257,234 @@ __device__ __forceinline__ void vjp_stream(Solver<G, 0>& sv, const dexr_sequence
   }
 }
 
+// ------------------------------------------------------------------------------------------------
+// packed streams (dexr_solve_sequences_packed / _packed_vjp): streams of any lengths, frames laid end to end
+// ------------------------------------------------------------------------------------------------
+// The argument checks of the packed calls: nullptr, or what is wrong.  Host code shared by the library and the host
+// emulation.  `tape` nullptr: the unrecorded forward.  offsets live on the device and are not read here.
+inline const char* packed_io_error(const dexr_table_t& t, const dexr_sequences_t& io, const dexr_sequences_tape_t* tape,
+                                   const dexr_params_t& prm, const int64_t* offsets, long long S, long long N) {
+  if (S < 0 || N < 0 || N > INT32_MAX) return "bad sizes: num_streams and num_frames must be >= 0, num_frames <= INT32_MAX";
+  if (!offsets) return "offsets (device [S+1]) are required";
+  if (!io.keypoints || !io.last_qpos || !io.robot_qpos_out) return "keypoints, last_qpos, robot_qpos_out required";
+  const bool use_filter = prm.lp_alpha >= 0.f && prm.lp_alpha <= 1.f;
+  if (use_filter && (!io.filter_state || !io.filter_init)) return "low-pass filter needs filter_state and filter_init";
+  if (t.n_fixed > 0 && !io.fixed_qpos) return "the robot has fixed joints but fixed_qpos is NULL";
+  if (tape) {
+    if (prm.preprocess != 0) return "raw-landmark pre-processing is not recorded: params.preprocess must be 0 with a tape";
+    if (!tape->qpos) return "tape->qpos is required";
+    if (t.loss == DEXR_LOSS_DEXPILOT && (!tape->projected || !io.projected))
+      return "DexPilot: the flag tape needs tape->projected and io->projected";
+  }
+  return nullptr;
+}
+
+inline const char* packed_io_error(const dexr_table_t& t, const dexr_sequences_vjp_t& io, const dexr_params_t& prm,
+                                   const int64_t* offsets, long long S, long long N) {
+  if (S < 0 || N < 0 || N > INT32_MAX) return "bad sizes: num_streams and num_frames must be >= 0, num_frames <= INT32_MAX";
+  if (!offsets) return "offsets (device [S+1]) are required";
+  return seq_vjp_io_error(t, io, prm);
+}
+
+// Where the packed streams lie: offsets [S+1] into the N frames.
+struct PackedLayout {
+  const int64_t* offsets;
+  long long S, N;
+};
+
+// Stream number s (-1: none) and frame range of stream i.  A malformed range reads as an empty stream, so no layout can
+// make a kernel reach outside its buffers.
+struct PackedStream {
+  long long s, first;
+  int len;
+};
+
+__device__ __forceinline__ PackedStream packed_stream(const PackedLayout& pk, long long i) {
+  PackedStream r{-1, 0, 0};
+  if (i < 0 || i >= pk.S) return r;
+  r.s = i;
+  const long long a = pk.offsets[i], b = pk.offsets[i + 1];
+  if (a >= 0 && a <= b && b <= pk.N) {
+    r.first = a;
+    r.len = (int)(b - a);  // (N <= INT32_MAX)
+  }
+  return r;
+}
+
+// The longer of the warp's stream lengths: every group of a warp walks the time loop that long (warp-wide shuffles inside
+// solve and vjp_front).
+template <int G>
+__device__ __forceinline__ int warp_steps(int len) {
+  if constexpr (G == 16) {
+    const int other = __shfl_xor_sync(0xffffffffu, len, 16);
+    return other > len ? other : len;
+  } else {
+    return len;
+  }
+}
+
+// solve_stream for one packed stream `ps` (ps.s < 0: none).  `works`: this group solves the stream (the owner, or the
+// helping half-warp in duo mode); `writes`: it stores results and state.  The warp loops to the longer of its groups'
+// lengths; a group past its end (or without a stream) solves a valid frame inactive -- its own last frame, or frame 0 --
+// with writes off.  Its state is stored at its own last frame, so the extra frames change nothing it wrote.  Per frame the
+// arithmetic is solve_stream's; a twin rather than a generalisation, which would move the machine code of the
+// rectangular sequences kernels.
+template <int G, int BW, bool REC>
+__device__ __forceinline__ void solve_packed_stream(Solver<G, BW>& sv, const dexr_sequences_t& io, const Dims& dm,
+                                                    const dexr_params_t& prm, const PackedStream& ps, bool works, bool writes,
+                                                    float* kpbuf, bool use_filter, float* tape_qpos, uint8_t* tape_proj) {
+  constexpr int KPL = (3 * DEXR_NUM_KEYPOINTS + G - 1) / G;
+  const int l = sv.l;
+  const int len = works && ps.s >= 0 ? ps.len : 0;
+  const int steps = warp_steps<G>(len);
+  if (steps == 0) return;
+  const bool has = len > 0;
+  writes = writes && has;
+  const long long sc = has ? ps.s : 0, f0 = has ? ps.first : 0;
+  const int tlast = has ? len - 1 : 0;
+  float last = 0.f, fy = 0.f;
+  int finit = 0;
+  if (has && sv.var >= 0) last = io.last_qpos[sc * dm.n_var + sv.var];
+  if (has && use_filter && l < dm.dof) fy = io.filter_state[sc * dm.dof + l];
+  if (has && use_filter) finit = io.filter_init[sc];
+  sv.lam_carry = (has && io.damping_state) ? io.damping_state[sc] : 0.f;
+  const float* kp_stream = io.keypoints + f0 * (3 * DEXR_NUM_KEYPOINTS);
+  float pre[KPL];
+#pragma unroll
+  for (int j = 0; j < KPL; ++j) {
+    const int e = l + j * G;
+    pre[j] = (e < 3 * DEXR_NUM_KEYPOINTS) ? kp_stream[e] : 0.f;
+  }
+  for (int t = 0; t < steps; ++t) {
+#pragma unroll
+    for (int j = 0; j < KPL; ++j) {
+      const int e = l + j * G;
+      if (e < 3 * DEXR_NUM_KEYPOINTS) kpbuf[e] = pre[j];
+    }
+    if (t + 1 < steps) {
+      const float* nxt = kp_stream + (long long)(t + 1 < tlast ? t + 1 : tlast) * (3 * DEXR_NUM_KEYPOINTS);
+#pragma unroll
+      for (int j = 0; j < KPL; ++j) {
+        const int e = l + j * G;
+        pre[j] = (e < 3 * DEXR_NUM_KEYPOINTS) ? nxt[e] : 0.f;
+      }
+    }
+    __syncwarp();
+    const bool act = t < len;
+    const long long fr = f0 + (t < tlast ? t : tlast);
+    FrameInputs in;
+    in.kp = kpbuf;
+    in.ref = nullptr;
+    in.fixed = dm.n_fixed > 0 ? io.fixed_qpos + fr * dm.n_fixed : nullptr;
+    in.last = nullptr;
+    in.projected = io.projected ? io.projected + sc * dm.len_proj : nullptr;
+    sv.x = last;
+    const int status = sv.solve(in, act);
+    last = sv.x;
+    const bool w = writes && act;
+    if constexpr (REC) {
+      if (w) {
+        if (sv.var >= 0) tape_qpos[fr * dm.n_var + sv.var] = last;
+        if (tape_proj && l < dm.len_proj) tape_proj[fr * dm.len_proj + l] = io.projected[sc * dm.len_proj + l];
+      }
+    }
+    float out = sv.q;
+    if (use_filter) {
+      fy = finit ? fmaf(prm.lp_alpha, out - fy, fy) : out;
+      finit = 1;
+      out = fy;
+    }
+    if (w) {
+      if (l < dm.dof) io.robot_qpos_out[fr * dm.dof + l] = out;
+      if (l == 0 && io.status_out) io.status_out[fr] = status;
+      if (t == tlast) {
+        if (sv.var >= 0) io.last_qpos[sc * dm.n_var + sv.var] = last;
+        if (use_filter && l < dm.dof) io.filter_state[sc * dm.dof + l] = fy;
+        if (use_filter && l == 0) io.filter_init[sc] = (uint8_t)finit;
+        if (io.damping_state && l == 0) io.damping_state[sc] = sv.lam_carry;
+      }
+    }
+    __syncwarp();
+  }
+}
+
+// vjp_stream for one packed stream `ps` (ps.s < 0: none), walked from its last frame to its first while the warp walks
+// t = steps - 1 .. 0; frames past the group's end run inactive on a valid frame and leave gy and c as they are.  A
+// stream of length 0 passes its state cotangents through.  Per frame the arithmetic is vjp_stream's.
+template <int G>
+__device__ __forceinline__ void vjp_packed_stream(Solver<G, 0>& sv, const dexr_sequences_vjp_t& io, const Dims& dm,
+                                                  const PackedStream& ps, bool owner, bool use_filter) {
+  const SharedTable& st = Solver<G, 0>::ST();
+  const int l = sv.l;
+  const bool isvar = sv.var >= 0, isjoint = l < dm.dof;
+  const bool valid = owner && ps.s >= 0;
+  const int len = valid ? ps.len : 0;
+  const int steps = warp_steps<G>(len);
+  const long long sc = valid ? ps.s : 0, f0 = len > 0 ? ps.first : 0;
+  const int tlast = len > 0 ? len - 1 : 0;
+  const float alpha = sv.prm.lp_alpha, nd = sv.prm.norm_delta;
+  float gy = 0.f, c = 0.f;
+  if (valid && isjoint && io.grad_filter_state_out) gy = io.grad_filter_state_out[sc * dm.dof + l];
+  if (valid && isvar && io.grad_last_qpos_out) c = io.grad_last_qpos_out[sc * dm.n_var + sv.var];
+  const bool finit = valid && use_filter && io.filter_init[sc];
+  for (int t = steps - 1; t >= 0; --t) {
+    const bool act = t < len;
+    const long long fr = f0 + (t < tlast ? t : tlast);
+    float gq = (act && isjoint && io.grad_robot_qpos) ? io.grad_robot_qpos[fr * dm.dof + l] : 0.f;
+    float gyn = gy;
+    if (use_filter) {
+      gyn += gq;
+      const bool init = t > 0 || finit;
+      gq = init ? alpha * gyn : gyn;
+      gyn = init ? (1.0f - alpha) * gyn : 0.f;
+    }
+    float gbar = gq;
+    if (dm.has_mimic) {
+      const int gcount = st.group_count[l];
+      float gx_ = 0.f;
+#pragma unroll
+      for (int k = 0; k < DEXR_MAX_GROUP; ++k) {
+        const bool v = isvar && k < gcount;
+        const float gv = gshfl<G>(gq, v ? st.group_lane[l][k] : l);
+        if (v) gx_ = fmaf(st.group_mult[l][k], gv, gx_);
+      }
+      gbar = gx_;
+    }
+    gbar = isvar ? gbar + c : 0.f;
+    float x = 0.f, xp = 0.f;
+    if (act && isvar) {
+      x = io.qpos[fr * dm.n_var + sv.var];
+      xp = t > 0 ? io.qpos[(fr - 1) * dm.n_var + sv.var] : io.last_qpos[sc * dm.n_var + sv.var];
+    }
+    const float clo = st.clip_lo[l], chi = st.clip_hi[l];
+    const float a = fminf(fmaxf(xp, clo), chi);
+    const bool passes = xp >= clo && xp <= chi;
+    FrameInputs in;
+    in.kp = io.keypoints + fr * (3 * DEXR_NUM_KEYPOINTS);
+    in.ref = nullptr;
+    in.fixed = dm.n_fixed > 0 ? io.fixed_qpos + fr * dm.n_fixed : nullptr;
+    in.last = nullptr;
+    in.projected = nullptr;
+    const VjpFront vf = vjp_front(sv, in, dm, x, a, gbar, nd, io.projected ? io.projected + fr * dm.len_proj : nullptr, act);
+    const VjpLane r = vjp_tail(sv, in, dm, vf, gbar, nullptr, act);
+    auto out = [&](float val) { return !r.finite ? __int_as_float(0x7fc00000) : val; };
+    const float cn = out(2.0f * nd * r.v) * (passes ? 1.0f : 0.f);
+    if (act) {
+      gy = gyn;
+      c = cn;
+      const int fixedi = st.fixed_index[l];
+      const float* const kpacc = sv.scf() + VjpScratch<G>::kKp;
+      if (fixedi >= 0 && io.grad_fixed_qpos) io.grad_fixed_qpos[fr * dm.n_fixed + fixedi] = out(gq - r.qbar);
+      if (io.grad_keypoints)
+        for (int e = l; e < 3 * DEXR_NUM_KEYPOINTS; e += G) io.grad_keypoints[fr * 3 * DEXR_NUM_KEYPOINTS + e] = out(kpacc[e]);
+      if (l == 0 && io.status_out) io.status_out[fr] = !r.finite ? DEXR_STATUS_NONFINITE : (r.bad ? DEXR_STATUS_NOT_PD : 0);
+    }
+    __syncwarp();
+  }
+  if (valid) {
+    if (isvar && io.grad_last_qpos) io.grad_last_qpos[sc * dm.n_var + sv.var] = c;
+    if (isjoint && io.grad_filter_state) io.grad_filter_state[sc * dm.dof + l] = gy;
+  }
+}
+
 }  // namespace dexr

@@ -154,3 +154,56 @@ def differentiable_retarget_sequences(seq, keypoints, state=None, fixed_qpos=Non
     new = cfg["new_state"]
     return out, StreamState(last_qpos=last, filter_state=filt, filter_init=new.filter_init, projected=new.projected,
                             damping=new.damping)
+
+
+class _DifferentiableRetargetPackedSequences(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, keypoints, fixed_qpos, last_qpos, filter_state, seq, cfg):
+        from .seq_retarget import StreamState
+
+        st, layout = cfg["state"], cfg["layout"]
+        new = StreamState(last_qpos=last_qpos.detach().clone(), filter_state=filter_state.detach().clone(),
+                          filter_init=st.filter_init.clone(), projected=None if st.projected is None else st.projected.clone(),
+                          damping=None if st.damping is None else st.damping.clone())
+        tape = seq.make_packed_sequence_tape(layout)
+        kp = keypoints.detach().contiguous()
+        fixed = None if fixed_qpos is None else fixed_qpos.detach().contiguous()
+        out, _ = seq.retarget_packed_sequences(kp, layout, new, fixed_qpos=fixed, tape=tape)
+        ctx.seq, ctx.tape, ctx.layout = seq, tape, layout
+        ctx.save_for_backward(kp, fixed, last_qpos.detach().contiguous(), st.filter_init.clone())
+        ctx.set_materialize_grads(False)
+        cfg["new_state"] = new
+        return out, new.last_qpos, new.filter_state
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g_out, g_last, g_filter):
+        keypoints, fixed, last0, finit0 = ctx.saved_tensors
+        c = (lambda g: None if g is None else g.contiguous())
+        g_kp, g_fixed, g_last0, g_filter0 = ctx.seq.retarget_packed_sequences_vjp(
+            keypoints, ctx.layout, ctx.tape, last0, finit0, grad_robot_qpos=c(g_out), grad_last_qpos=c(g_last),
+            grad_filter_state=c(g_filter), fixed_qpos=fixed)
+        return g_kp, g_fixed, g_last0, g_filter0, None, None
+
+
+def differentiable_retarget_packed_sequences(seq, keypoints, layout, state=None, fixed_qpos=None, *, raw_hand=None):
+    """(robot_qpos [N,dof], new_state) = `seq.retarget_packed_sequences(keypoints, layout, state, fixed_qpos)` for streams of
+    any lengths packed end to end (`seq.pack_streams`), differentiable in `keypoints` [N,21,3], `fixed_qpos` [N,n_fixed],
+    `state.last_qpos` and `state.filter_state` ([S,...]).  The contract of `differentiable_retarget_sequences`: `state` is
+    not modified, and the returned state carries the graph across chunks.  backward() is one
+    `retarget_packed_sequences_vjp` launch.  Raw detector landmarks (`raw_hand`) are solved but not differentiated."""
+    from .seq_retarget import StreamState
+
+    state = seq.make_stream_state(layout.num_streams) if state is None else state
+    if raw_hand is not None:
+        if any(t is not None and t.requires_grad for t in (keypoints, fixed_qpos, state.last_qpos, state.filter_state)):
+            raise ValueError("raw_hand: raw-landmark pre-processing is not differentiated; pre-process the keypoints "
+                             "(dexr_preprocess_keypoints) and pass them without raw_hand")
+        new = StreamState(**{k: (None if getattr(state, k) is None else getattr(state, k).clone()) for k in StreamState._FIELDS})
+        return seq.retarget_packed_sequences(keypoints, layout, new, fixed_qpos=fixed_qpos, raw_hand=raw_hand)
+    cfg = dict(state=state, layout=layout)
+    out, last, filt = _DifferentiableRetargetPackedSequences.apply(keypoints, fixed_qpos, state.last_qpos,
+                                                                   state.filter_state, seq, cfg)
+    new = cfg["new_state"]
+    return out, StreamState(last_qpos=last, filter_state=filt, filter_init=new.filter_init, projected=new.projected,
+                            damping=new.damping)

@@ -11,6 +11,8 @@ inside ONE kernel launch (`dexr_solve_sequences`): a group of lanes owns a strea
 With a `SequenceTape` the same launch also records every frame's unfiltered solution (and DexPilot flags), and
 `retarget_sequences_vjp()` backpropagates through all T frames of every stream in one launch
 (`dexr_solve_sequences_vjp`; `objective.differentiable_retarget_sequences` wraps both for autograd).
+`retarget_packed_sequences()` / `retarget_packed_sequences_vjp()` do the same for streams of different lengths laid end to
+end (`PackedStreams`, the cu_seqlens layout): recorded clips of any length in one launch, no padding.
 """
 from __future__ import annotations
 
@@ -76,6 +78,41 @@ class SequenceTape:
 
     qpos: "torch.Tensor"                 # [S, T, opt_dof] float32: every frame's unfiltered solution
     projected: Optional["torch.Tensor"]  # [S, T, len_proj] uint8: the DexPilot flags after every frame, or None
+
+
+@dataclass
+class PackedStreams:
+    """Layout of S streams of any lengths packed end to end (`SeqRetargeting.pack_streams`): stream s owns frames
+    offsets[s] .. offsets[s+1]-1 of every per-frame tensor [N,...]; per-stream tensors (`StreamState`) stay [S,...]."""
+
+    lengths: tuple                # S host ints
+    offsets: "torch.Tensor"       # [S+1] int64 on the device
+
+    @property
+    def num_streams(self) -> int:
+        return len(self.lengths)
+
+    @property
+    def num_frames(self) -> int:
+        return int(sum(self.lengths))
+
+    def split(self, t):
+        """Per-stream views of a packed tensor [N,...]: a list of S tensors [len_s,...]."""
+        if int(t.shape[0]) != self.num_frames:
+            raise ValueError(f"packed tensor has {int(t.shape[0])} frames, the layout {self.num_frames}")
+        return list(t.split(list(self.lengths), dim=0))
+
+
+def _checker(dev):
+    """The shape / dtype / device check of the stream calls' tensor arguments; returns the data pointer."""
+
+    def chk(t, shape, dtype, name):
+        if t.device != dev or t.dtype != dtype or not t.is_contiguous() or tuple(t.shape) != tuple(shape):
+            raise ValueError(f"{name}: expected contiguous {dtype} tensor of shape {tuple(shape)} on {dev}, "
+                             f"got {t.dtype} {tuple(t.shape)} on {t.device}")
+        return t.data_ptr()
+
+    return chk
 
 
 def _quat_to_matrix(q):
@@ -399,4 +436,151 @@ class SeqRetargeting:
         p = opt.params(clip_init=True, lp_alpha=self.low_pass_alpha)
         N.check(eng.lib.dexr_solve_sequences_vjp(eng.handle, C.byref(p), C.byref(io), S, T, C.c_void_p(s.cuda_stream)),
                 "dexr_solve_sequences_vjp")
+        return g_kp, g_fixed, g_last, g_filter
+
+    # ------------------------------------------------------------------------------ packed streams (any lengths)
+    def pack_streams(self, lengths) -> PackedStreams:
+        """The layout of S streams of the given frame counts (0 allowed), packed end to end in that order.  Validated on
+        the host; the offsets are uploaded without synchronising (a pinned host copy).  Build it once per batch of clips
+        and pass it to every packed call on them.  The streams are dealt to warps in this order; dealing them longest first
+        measured no faster on an H100 (DESIGN.md section 3.11)."""
+        import torch
+
+        lens = np.asarray(lengths)
+        if lens.ndim != 1 or (lens.size and not np.issubdtype(lens.dtype, np.integer)):
+            raise ValueError(f"lengths must be a 1-D sequence of ints, got {lens.dtype} of shape {lens.shape}")
+        lens = lens.astype(np.int64)
+        if (lens < 0).any():
+            raise ValueError("stream lengths must be >= 0")
+        if int(lens.sum()) > np.iinfo(np.int32).max:
+            raise ValueError("at most 2**31 - 1 frames in one packed batch")
+        offsets = np.zeros(lens.size + 1, np.int64)
+        np.cumsum(lens, out=offsets[1:])
+        dev = torch.device("cuda", self.optimizer.device_index)
+        return PackedStreams(lengths=tuple(int(v) for v in lens),
+                             offsets=torch.from_numpy(offsets).pin_memory().to(dev, non_blocking=True))
+
+    def make_packed_sequence_tape(self, layout: PackedStreams) -> SequenceTape:
+        """Empty tape buffers for a recorded `retarget_packed_sequences` call: qpos [N,opt_dof], projected [N,len_proj]."""
+        import torch
+
+        opt = self.optimizer
+        dev = torch.device("cuda", opt.device_index)
+        N_ = layout.num_frames
+        len_proj = opt._objective_spec().len_proj
+        return SequenceTape(
+            qpos=torch.empty((N_, opt.opt_dof), dtype=torch.float32, device=dev),
+            projected=(torch.empty((N_, len_proj), dtype=torch.uint8, device=dev)
+                       if opt.retargeting_type == "DEXPILOT" else None))
+
+    def retarget_packed_sequences(self, keypoints, layout: PackedStreams, state: Optional[StreamState] = None,
+                                  fixed_qpos=None, out=None, status_out=None, stream=None, raw_hand=None,
+                                  tape: Optional[SequenceTape] = None):
+        """`retarget_sequences` for S streams of any lengths in one launch (`dexr_solve_sequences_packed`): keypoints
+        [N,21,3] float32 CUDA tensor with stream s at frames layout.offsets[s] .. offsets[s+1]-1 (`pack_streams`),
+        fixed_qpos [N,n_fixed].  Returns (robot_qpos [N,dof], state); `state` ([S,...], `make_stream_state(S)`) is updated
+        in place, each stream ending at its own last frame (a stream of length 0 keeps its state), so chunks of the same
+        clips chain exactly.  Every stream's results are bit-identical to a `retarget_sequences` call on it alone.
+        `tape` (`make_packed_sequence_tape(layout)`) records the call for `retarget_packed_sequences_vjp`."""
+        if tape is not None and raw_hand is not None:
+            raise ValueError("raw_hand with a tape: raw-landmark pre-processing is not differentiated; pre-process the "
+                             "keypoints (dexr_preprocess_keypoints) and record the call without raw_hand")
+        import torch
+
+        opt = self.optimizer
+        eng = opt.engine()
+        dev = torch.device("cuda", eng.device)
+        S, N_ = layout.num_streams, layout.num_frames
+        chk = _checker(dev)
+        if state is None:
+            state = self.make_stream_state(S)
+        io = N.DexrSequences()
+        io.keypoints = chk(keypoints, (N_, N.NUM_KEYPOINTS, 3), torch.float32, "keypoints")
+        nf = len(opt.idx_pin2fixed)
+        if nf:
+            if fixed_qpos is None:
+                raise ValueError(f"Optimizer has {nf} joints but no fixed_qpos is given")
+            io.fixed_qpos = chk(fixed_qpos, (N_, nf), torch.float32, "fixed_qpos")
+        io.last_qpos = chk(state.last_qpos, (S, opt.opt_dof), torch.float32, "state.last_qpos")
+        io.filter_state = chk(state.filter_state, (S, opt.robot.dof), torch.float32, "state.filter_state")
+        io.filter_init = chk(state.filter_init, (S,), torch.uint8, "state.filter_init")
+        if state.projected is not None:
+            io.projected = chk(state.projected, (S, state.projected.shape[1]), torch.uint8, "state.projected")
+        if state.damping is not None:
+            io.damping_state = chk(state.damping, (S,), torch.float32, "state.damping")
+        if out is None:
+            out = torch.empty((N_, opt.robot.dof), dtype=torch.float32, device=dev)
+        io.robot_qpos_out = chk(out, (N_, opt.robot.dof), torch.float32, "out")
+        if status_out is not None:
+            io.status_out = chk(status_out, (N_,), torch.int32, "status_out")
+        tp = None
+        if tape is not None:
+            tp = N.DexrSequencesTape()
+            tp.qpos = chk(tape.qpos, (N_, opt.opt_dof), torch.float32, "tape.qpos")
+            if tape.projected is not None:
+                tp.projected = chk(tape.projected, (N_, opt._objective_spec().len_proj), torch.uint8, "tape.projected")
+        offsets = chk(layout.offsets, (S + 1,), torch.int64, "layout.offsets")
+        s = stream if stream is not None else torch.cuda.current_stream(dev)
+        p = opt.params(clip_init=True, lp_alpha=self.low_pass_alpha, raw_hand=raw_hand)
+        N.check(eng.lib.dexr_solve_sequences_packed(eng.handle, C.byref(p), C.byref(io), None if tp is None else C.byref(tp),
+                                                    C.c_void_p(offsets), S, N_,
+                                                    C.c_void_p(s.cuda_stream)), "dexr_solve_sequences_packed")
+        return out, state
+
+    def retarget_packed_sequences_vjp(self, keypoints, layout: PackedStreams, tape: SequenceTape, last_qpos0, filter_init0,
+                                      grad_robot_qpos=None, grad_last_qpos=None, grad_filter_state=None, fixed_qpos=None,
+                                      grad_keypoints_out=None, grad_fixed_qpos_out=None, grad_last_qpos_out=None,
+                                      grad_filter_state_out=None, status_out=None, stream=None):
+        """`retarget_sequences_vjp` for a recorded `retarget_packed_sequences` call, one launch
+        (`dexr_solve_sequences_packed_vjp`): per-frame tensors [N,...] (keypoints, fixed_qpos, tape, grad_robot_qpos,
+        status_out and the returned grad_keypoints / grad_fixed_qpos), per-stream ones [S,...] (last_qpos0, filter_init0,
+        grad_last_qpos, grad_filter_state and the returned initial-state gradients).  A stream of length 0 passes its
+        state cotangents through.  Nothing is synchronised."""
+        import torch
+
+        opt = self.optimizer
+        eng = opt.engine()
+        dev = torch.device("cuda", eng.device)
+        S, N_ = layout.num_streams, layout.num_frames
+        n, dof, nf = opt.opt_dof, opt.robot.dof, len(opt.idx_pin2fixed)
+        chk = _checker(dev)
+
+        def out(t, shape, name):
+            t = torch.empty(shape, dtype=torch.float32, device=dev) if t is None else t
+            return t, chk(t, shape, torch.float32, name)
+
+        io = N.DexrSequencesVjp()
+        io.keypoints = chk(keypoints, (N_, N.NUM_KEYPOINTS, 3), torch.float32, "keypoints")
+        if nf:
+            if fixed_qpos is None:
+                raise ValueError(f"Optimizer has {nf} fixed joints but no fixed_qpos is given")
+            io.fixed_qpos = chk(fixed_qpos, (N_, nf), torch.float32, "fixed_qpos")
+        io.last_qpos = chk(last_qpos0, (S, n), torch.float32, "last_qpos0")
+        io.filter_init = chk(filter_init0, (S,), torch.uint8, "filter_init0")
+        io.qpos = chk(tape.qpos, (N_, n), torch.float32, "tape.qpos")
+        if tape.projected is not None:
+            io.projected = chk(tape.projected, (N_, opt._objective_spec().len_proj), torch.uint8, "tape.projected")
+        if grad_robot_qpos is not None:
+            io.grad_robot_qpos = chk(grad_robot_qpos, (N_, dof), torch.float32, "grad_robot_qpos")
+        if grad_last_qpos is not None:
+            io.grad_last_qpos_out = chk(grad_last_qpos, (S, n), torch.float32, "grad_last_qpos")
+        if grad_filter_state is not None:
+            io.grad_filter_state_out = chk(grad_filter_state, (S, dof), torch.float32, "grad_filter_state")
+        g_kp, io.grad_keypoints = out(grad_keypoints_out, (N_, N.NUM_KEYPOINTS, 3), "grad_keypoints_out")
+        g_fixed = None
+        if nf:
+            g_fixed, io.grad_fixed_qpos = out(grad_fixed_qpos_out, (N_, nf), "grad_fixed_qpos_out")
+        g_last, io.grad_last_qpos = out(grad_last_qpos_out, (S, n), "grad_last_qpos_out")
+        g_filter, io.grad_filter_state = out(grad_filter_state_out, (S, dof), "grad_filter_state_out")
+        if status_out is not None:
+            io.status_out = chk(status_out, (N_,), torch.int32, "status_out")
+        offsets = chk(layout.offsets, (S + 1,), torch.int64, "layout.offsets")
+        if N_ == 0:  # (the library does nothing for 0 frames: every stream is empty and passes its cotangents through)
+            g_last.copy_(grad_last_qpos) if grad_last_qpos is not None else g_last.zero_()
+            g_filter.copy_(grad_filter_state) if grad_filter_state is not None else g_filter.zero_()
+        s = stream if stream is not None else torch.cuda.current_stream(dev)
+        p = opt.params(clip_init=True, lp_alpha=self.low_pass_alpha)
+        N.check(eng.lib.dexr_solve_sequences_packed_vjp(eng.handle, C.byref(p), C.byref(io), C.c_void_p(offsets), S, N_,
+                                                        C.c_void_p(s.cuda_stream)),
+                "dexr_solve_sequences_packed_vjp")
         return g_kp, g_fixed, g_last, g_filter

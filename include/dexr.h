@@ -389,6 +389,31 @@ size_t dexr_jacobian_sizeof(void);
 int dexr_solve_jacobian(const dexr_robot_t* robot, const dexr_params_t* params, const dexr_jacobian_t* io,
                         int64_t num_frames, void* cuda_stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Packed streams: S streams of ANY lengths in one launch, their frames laid end to end (the cu_seqlens layout).  Stream s
+ * owns frames offsets[s] .. offsets[s+1]-1 of every per-frame array; N = num_frames.  The buffer structs are those of the
+ * rectangular calls with these shapes:
+ *   dexr_sequences_t:      keypoints [N,21,3], fixed_qpos [N,n_fixed], robot_qpos_out [N,dof], status_out [N];
+ *                          last_qpos [S,n_var], filter_state [S,dof], filter_init [S], projected [S,len_proj],
+ *                          damping_state [S] (per stream, as before)
+ *   dexr_sequences_tape_t: qpos [N,n_var], projected [N,len_proj]
+ *   dexr_sequences_vjp_t:  keypoints, fixed_qpos, qpos, projected, grad_robot_qpos, grad_keypoints, grad_fixed_qpos,
+ *                          status_out [N,...]; last_qpos, filter_init, grad_last_qpos_out, grad_filter_state_out,
+ *                          grad_last_qpos, grad_filter_state [S,...]
+ * Per stream everything is exactly what dexr_solve_sequences / _tape / _vjp do (a stream's results and final state are
+ * bit-identical to a rectangular call on that stream alone).  A stream of length 0 leaves its state untouched; in the
+ * backward its state cotangents pass through unchanged.  `tape` NULL: not recorded (raw landmarks, params.preprocess,
+ * are accepted only then).  Streams are dealt to warps in index order.  offsets is a DEVICE array and is not checked on
+ * the host: a stream whose range is malformed (offsets[s] < 0, offsets[s] > offsets[s+1] or offsets[s+1] > N) is treated
+ * as an empty stream, so no layout makes the kernels read or write out of range.
+ * num_frames == 0 does nothing.  Asynchronous on `cuda_stream`, allocates nothing.  All pointers are DEVICE pointers.
+ * ------------------------------------------------------------------------------------------- */
+int dexr_solve_sequences_packed(const dexr_robot_t* robot, const dexr_params_t* params, const dexr_sequences_t* io,
+                                const dexr_sequences_tape_t* tape /* NULL: not recorded */,
+                                const int64_t* offsets /* device [S+1] */, int64_t num_streams, int64_t num_frames, void* cuda_stream);
+int dexr_solve_sequences_packed_vjp(const dexr_robot_t* robot, const dexr_params_t* params, const dexr_sequences_vjp_t* io,
+                                    const int64_t* offsets, int64_t num_streams, int64_t num_frames, void* cuda_stream);
+
 #ifdef __cplusplus
 }
 #endif

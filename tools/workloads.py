@@ -151,3 +151,15 @@ def digest(*arrays):
         if a is not None:
             h.update(np.ascontiguousarray(a).tobytes())
     return h.hexdigest()[:16]
+
+
+def ragged_streams(S, lo=60, hi=300, seed=STREAM_SEED):
+    """(keypoints [N,21,3] f32 packed end to end, lengths [S] int64): stream s is the first lengths[s] recorded frames with
+    its own 2 mm keypoint offsets (wrist kept at 0), as in `streams`; lengths are seeded, uniform over [lo, hi]."""
+    traj = np.load(TRAJECTORY).astype(np.float32)
+    rng = np.random.RandomState(seed)
+    lengths = rng.randint(lo, hi + 1, size=S).astype(np.int64)
+    offs = rng.randn(S, 1, 21, 3).astype(np.float32) * 0.002
+    kp = np.concatenate([traj[:n] + offs[s] for s, n in enumerate(lengths)]) if S else np.zeros((0, 21, 3), np.float32)
+    kp[:, 0] = 0
+    return np.ascontiguousarray(kp), lengths
