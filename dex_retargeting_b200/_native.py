@@ -18,6 +18,7 @@ TABLE_MAGIC = 0x31525844
 STATUS_MAXITER = 1 << 24
 STATUS_NONFINITE = 1 << 25
 STATUS_NOT_PD = 1 << 26
+STATUS_MISSING = 1 << 27
 
 _f, _i, _u = C.c_float, C.c_int32, C.c_uint32
 
@@ -116,6 +117,16 @@ class DexrJacobian(C.Structure):
     ]
 
 
+class DexrSmooth(C.Structure):
+    """Mirror of `dexr_smooth_t`: buffers of one offline smoothing launch (`dexr_smooth_sequences_packed`)."""
+
+    _fields_ = [
+        ("keypoints", C.c_void_p), ("fixed_qpos", C.c_void_p), ("last_qpos", C.c_void_p), ("projected", C.c_void_p),
+        ("qpos_init", C.c_void_p), ("qpos_out", C.c_void_p), ("robot_qpos_out", C.c_void_p), ("status_out", C.c_void_p),
+        ("cost_out", C.c_void_p), ("smooth_weight", _f), ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t),
+    ]
+
+
 class DexrGroup(C.Structure):
     """Mirror of `dexr_group_t`: one (robot, batch) group of a mixed-robot launch."""
 
@@ -138,6 +149,7 @@ EXPORTS = [
     "dexr_preprocess_keypoints", "dexr_eval_sizeof", "dexr_eval_objective", "dexr_vjp_sizeof", "dexr_solve_vjp",
     "dexr_sequences_tape_sizeof", "dexr_solve_sequences_tape", "dexr_sequences_vjp_sizeof", "dexr_solve_sequences_vjp",
     "dexr_jacobian_sizeof", "dexr_solve_jacobian", "dexr_solve_sequences_packed", "dexr_solve_sequences_packed_vjp",
+    "dexr_smooth_sizeof", "dexr_smooth_workspace_bytes", "dexr_smooth_sequences_packed",
 ]
 
 _LIB = None
@@ -240,6 +252,16 @@ def load():
     elif not os.environ.get("DEXR_LIBRARY"):
         raise DexrError(f"{path} does not export dexr_solve_sequences_packed: rebuild it "
                         "(python -m dex_retargeting_b200.build --force)")
+    if hasattr(lib, "dexr_smooth_sizeof"):
+        lib.dexr_smooth_sizeof.restype = C.c_size_t
+        if lib.dexr_smooth_sizeof() != C.sizeof(DexrSmooth):
+            raise DexrError("dexr_smooth_t layout mismatch between library and binding (stale DEXR_LIBRARY?)")
+        lib.dexr_smooth_workspace_bytes.argtypes = [C.c_void_p, C.c_int64]
+        lib.dexr_smooth_workspace_bytes.restype = C.c_size_t
+        lib.dexr_smooth_sequences_packed.argtypes = [C.c_void_p, C.POINTER(DexrParams), C.POINTER(DexrSmooth), C.c_void_p,
+                                                     C.c_int64, C.c_int64, C.c_void_p]
+    elif not os.environ.get("DEXR_LIBRARY"):
+        raise DexrError(f"{path} does not export dexr_smooth_sizeof: rebuild it (python -m dex_retargeting_b200.build --force)")
     # (an older A/B library named by DEXR_LIBRARY reads a prefix of the buffer structs -- fields are only ever appended -- so
     # the single-robot entry points still work with it; dexr_solve_frames_multi, whose groups embed the struct, does not)
     _LIB = lib

@@ -487,6 +487,37 @@ __global__ void __launch_bounds__(kEvalWarps * 32, G == 16 ? 2 : 1) dexr_packed_
 }
 
 // ------------------------------------------------------------------------------------------------
+// offline smoothing of packed streams: the packed sequence VJP's launch shape and stream slots, one stream per group of G lanes
+// ------------------------------------------------------------------------------------------------
+struct SmoothArgs {
+  const dexr_table_t* table;
+  dexr_params_t prm;  // norm_delta holds the smoothing weight w
+  dexr_smooth_t io;
+  long long S;
+  Dims dm;
+  int scratch_off;
+};
+
+template <int G>
+__global__ void __launch_bounds__(kEvalWarps * 32, G == 16 ? 2 : 1) dexr_smooth_kernel(const SmoothArgs a, const PackedLayout pk) {
+  load_shared_table(*reinterpret_cast<SharedTable*>(dsmem), a.table);
+  __syncthreads();
+  constexpr int GPW = 32 / G;
+  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
+  const int lane = threadIdx.x & 31;
+  const int gid = warp * GPW + lane / G;
+  Solver<G, 0> sv;
+  sv.init(a.table, a.dm, (uint32_t)(a.scratch_off + gid * VjpScratch<G>::kFloats * 4), a.prm, lane);
+  float* const ws = static_cast<float*>(a.io.workspace);
+  // one stream per warp: a 16-lane warp's second group idles (measured no slower than two streams per warp, whose outer
+  // iteration counts differ, and 1.75x faster on Allegro clips; DESIGN.md 3.12)
+  for (long long base = 0; base < a.S; base += (long long)gridDim.x * kEvalWarps) {
+    const PackedStream ps = packed_stream(pk, base + (long long)warp * gridDim.x + blockIdx.x);
+    smooth_packed_stream(sv, a.io, a.dm, a.prm, ps, lane < G, ws);
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
 // keypoint pre-processing (single_hand_detector.py:100-103, 130-158): one thread per frame for the 3x3 frame,
 // tile staged through shared memory so that global loads / stores are coalesced 16-byte accesses
 // ------------------------------------------------------------------------------------------------
@@ -1477,6 +1508,56 @@ extern "C" int dexr_solve_sequences_packed_vjp(const dexr_robot_t* robot, const 
   const PackedLayout pk{offsets, num_streams, num_frames};
   return eval_lanes(r->host) == 16 ? launch_packed_seq_vjp<16>(r, params, io, pk, stream)
                                    : launch_packed_seq_vjp<32>(r, params, io, pk, stream);
+}
+
+// dexr_smooth_sequences_packed: dexr_packed_seq_vjp_kernel's CTA and occupancy rule, one stream per warp, the smoothing
+// weight passed in params.norm_delta.
+template <int G>
+static int launch_smooth(dexr_robot* r, const dexr_params_t* prm, const dexr_smooth_t* io, const PackedLayout& pk,
+                         cudaStream_t stream) {
+  SmoothArgs a{};
+  a.table = r->table_dev;
+  a.prm = *prm;
+  if (!(io->smooth_weight < 0.f)) a.prm.norm_delta = io->smooth_weight;
+  a.io = *io;
+  a.S = pk.S;
+  a.dm = make_dims(r->host);
+  a.scratch_off = round_up((int)sizeof(SharedTable), 16);
+  constexpr int GPW = 32 / G;
+  const int smem = a.scratch_off + kEvalWarps * GPW * VjpScratch<G>::kFloats * 4;
+  auto kern = dexr_smooth_kernel<G>;
+  CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  int per_sm = 1;
+  if (int e = eval_ctas_per_sm(kern, smem, &per_sm)) return e;
+  const long long ctas = pk.S;
+  const int grid = (int)std::min<long long>(ctas, (long long)r->num_sms * per_sm);
+  kern<<<grid, kEvalWarps * 32, smem, stream>>>(a, pk);
+  CUDA_TRY(cudaGetLastError());
+  {
+    std::lock_guard<std::mutex> lk(r->info_mu);
+    r->last = dexr_launch_info_t{grid, kEvalWarps * 32, smem, 0, G, kEvalWarps, r->last.kernels_launched + 1};
+  }
+  return 0;
+}
+
+extern "C" size_t dexr_smooth_sizeof(void) { return sizeof(dexr_smooth_t); }
+
+extern "C" size_t dexr_smooth_workspace_bytes(const dexr_robot_t* robot, int64_t num_frames) {
+  return robot ? smooth_workspace_bytes(robot->host, num_frames) : 0;
+}
+
+extern "C" int dexr_smooth_sequences_packed(const dexr_robot_t* robot, const dexr_params_t* params, const dexr_smooth_t* io,
+                                            const int64_t* offsets, int64_t num_streams, int64_t num_frames, void* cuda_stream) {
+  if (!robot || !params || !io) return fail(DEXR_E_INVALID, "dexr_smooth_sequences_packed: null argument");
+  if (const char* msg = smooth_io_error(robot->host, *io, *params, offsets, num_streams, num_frames))
+    return fail(DEXR_E_INVALID, "%s", msg);
+  if (int e = check_params(params)) return e;
+  if (num_streams == 0 || num_frames == 0) return 0;
+  DEVICE_SCOPE(robot->device);
+  dexr_robot* r = const_cast<dexr_robot*>(robot);
+  cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
+  const PackedLayout pk{offsets, num_streams, num_frames};
+  return eval_lanes(r->host) == 16 ? launch_smooth<16>(r, params, io, pk, stream) : launch_smooth<32>(r, params, io, pk, stream);
 }
 
 extern "C" {

@@ -1778,63 +1778,22 @@ __device__ __forceinline__ void vjp_column(const Solver<G, 0>& sv, int k, float&
   }
 }
 
-// What vjp_tail hands back to its driver, per lane: v (H_ff^-1 gbar_f on this lane's variable, 0 elsewhere), the fixed-joint
-// term H_q[c, :] . M v of a fixed lane (its cotangent is -qbar), and the frame's finite / not-positive-definite verdicts
-// (group-uniform).  The keypoint cotangents are in the scratch's kKp accumulator.
-struct VjpLane {
-  float v, qbar;
-  bool finite, bad;
-};
-
-// What vjp_front leaves for vjp_tail besides the scratch (H_q in kH, the factor in kA, the flags in kFlags): whether this
-// lane's variable is free, and the frame's finite / not-positive-definite verdicts (group-uniform).
-struct VjpFront {
-  bool free_, finite, bad;
-};
-
-// The implicit-function VJP of one frame is vjp_front once, then vjp_tail once per cotangent: vjp_frame (dexr_solve_vjp) and
-// vjp_stream (dexr_solve_sequences_vjp) run one tail, jacobian_frame (dexr_solve_jacobian) one per free variable.
-//
-// The per-frame front: the point x, the anchor x0 of this lane's variable come from the driver, with norm_delta `nd`
-// (0: no regulariser) and the frame's DexPilot flags `proj` (read into the scratch; nullptr = all 0); `gbar` only takes
-// part in the finiteness verdict.  Prepares the targets on the private flag copy, runs FK, builds the gradient, the active
-// set and the exact H_q, folds the mimic joints, freezes the active rows and factorises the free block in place in kA.  The
-// caller's flags are never written.
+// The data part of the exact Hessian and gradient at the point the group's scratch holds (targets in kFr, links of the FK at
+// x in lp(0), this lane's world axis and origin in sv.a / sv.p): H_q (loss curvature J^T (d2h/dr2) J plus the kinematic
+// curvature, column per lane) is written to the scratch's kH, and M^T g_q -- the gradient of L folded onto the variables
+// (meaningful on variable lanes only) -- is returned.  Shared by vjp_front and the smoother's forward sweep.  `kin` false leaves
+// the kinematic curvature out of H_q: the Gauss-Newton model J^T (d2h/dr2) J, positive semi-definite (the smoother's fallback
+// when the exact model is indefinite); the gradient is the same.
 template <int G>
-__device__ __forceinline__ VjpFront vjp_front(Solver<G, 0>& sv, const FrameInputs& in_, const Dims& dm, float x, float x0,
-                                              float gbar, float nd, const uint8_t* proj, bool active) {
+__device__ __forceinline__ float exact_grad_hq(Solver<G, 0>& sv, const Dims& dm, bool kin = true) {
   using VS = VjpScratch<G>;
   constexpr int NP = G;
   const SharedTable& st = Solver<G, 0>::ST();
-  const int l = sv.l, lane = sv.lane, dof = dm.dof, m = dm.n_res;
+  const int l = sv.l, dof = dm.dof, m = dm.n_res;
   const bool isvar = sv.var >= 0;
   float* const hq = sv.scf() + VS::kH;
-  float* const A = sv.scf() + VS::kA;
-  uint8_t* const flags = reinterpret_cast<uint8_t*>(sv.scf() + VS::kFlags);
 
-  // ---- targets (flags on the private copy), FK at x
-  const int fixedi = st.fixed_index[l];
-  sv.qfix = (active && fixedi >= 0) ? in_.fixed[fixedi] : 0.f;
-  sv.x = x;
-  if (l < dm.len_proj) flags[l] = (active && proj) ? proj[l] : (uint8_t)0;
-  __syncwarp();
-  FrameInputs in = in_;
-  in.projected = dm.len_proj > 0 ? flags : nullptr;
-  bool finite = isfinite(x) && isfinite(x0) && isfinite(sv.qfix) && isfinite(gbar);
-  const bool ok_targets = sv.prepare_targets(in, active);
-  finite = !gany<G>(!finite, lane) && ok_targets;
-  __syncwarp();
-  sv.q = sv.compose_q(x);
-  {
-    float R[9];
-    sv.fk(sv.q, R, sv.p);
-    sv.write_world_links();
-    sv.write_links(R, sv.p, 0);
-    sv.set_world_axis(R);
-  }
-  __syncwarp();
-
-  // ---- gradient of F and H_q, one residual per pass: loss curvature J^T (d2h/dr2) J, then the kinematic curvature
+  // ---- gradient of L and H_q, one residual per pass: loss curvature J^T (d2h/dr2) J, then the kinematic curvature
   const float beta = sv.prm.huber_delta, inv_beta = sv.inv_beta;
   const bool pos_loss = dm.loss == DEXR_LOSS_POSITION;
   float H[NP];
@@ -1898,13 +1857,13 @@ __device__ __forceinline__ VjpFront vjp_front(Solver<G, 0>& sv, const FrameInput
         const bool up = (sv.anc >> i) & 1u, dn = (sv.desc >> i) & 1u;
         const float vu = fmaf(ai.x, t0, fmaf(ai.y, t1, ai.z * t2));
         const float vd = fmaf(ar0, ti_.x, fmaf(ar1, ti_.y, ar2 * ti_.z));
-        H[i] += up ? vu : (dn ? vd : 0.f);
+        H[i] += kin ? (up ? vu : (dn ? vd : 0.f)) : 0.f;
       }
     }
   }
 #pragma unroll
   for (int i = 0; i < NP; ++i) hq[i * NP + l] = H[i];
-  // g_x = M^T g_q + 2 norm_delta (x - a), as in evaluate_frame
+  // g_x = M^T g_q, as in evaluate_frame
   if (dm.has_mimic) {
     const int gcount = st.group_count[l];
     float gx_ = 0.f;
@@ -1916,30 +1875,40 @@ __device__ __forceinline__ VjpFront vjp_front(Solver<G, 0>& sv, const FrameInput
     }
     g = gx_;
   }
-  g = isvar ? fmaf(2.0f * nd, x - x0, g) : 0.f;
+  return g;
+}
 
-  // ---- active set (the solver's rule at its widened bounds), then A = the free block of M^T H_q M + 2 norm_delta I
-  const bool act = isvar && ((x <= sv.lo && g > -kGradNoise) || (x >= sv.hi && g < kGradNoise));
-  const bool free_ = isvar && !act;
-  const unsigned fmask = gballot<G>(free_, lane);
-  __syncwarp();
-  {
-    const int gca = free_ ? st.group_count[l] : 0;
-    for (int c = 0; c < dof; ++c) {
-      float h = c == l ? 1.0f : 0.f;
-      if (free_ && ((fmask >> c) & 1u)) {
-        h = c == l ? 2.0f * nd : 0.f;
-        const int gcb = st.group_count[c];
-        for (int fb = 0; fb < gcb; ++fb) {
-          const float* col = hq + st.group_lane[c][fb] * NP;
-          const float mb = st.group_mult[c][fb];
-          for (int fa = 0; fa < gca; ++fa) h = fmaf(mb * st.group_mult[l][fa], col[st.group_lane[l][fa]], h);
-        }
+// Row l of A = the free block of M^T H_q M + diag I (H_q in the scratch's kH, M the scatter + mimic map: lane c's variable
+// feeds the joints st.group_lane[c][.] with multipliers st.group_mult[c][.]), identity rows and columns where a variable is
+// not free (`fmask`, group-wide) or a lane is not a variable.  Shared by vjp_front (diag = 2 norm_delta) and the smoother.
+template <int G>
+__device__ __forceinline__ void fold_free_block(const Solver<G, 0>& sv, const Dims& dm, float* A, bool free_, unsigned fmask,
+                                                float diag) {
+  constexpr int NP = G;
+  const SharedTable& st = Solver<G, 0>::ST();
+  const int l = sv.l, dof = dm.dof;
+  const float* const hq = sv.scf() + VjpScratch<G>::kH;
+  const int gca = free_ ? st.group_count[l] : 0;
+  for (int c = 0; c < dof; ++c) {
+    float h = c == l ? 1.0f : 0.f;
+    if (free_ && ((fmask >> c) & 1u)) {
+      h = c == l ? diag : 0.f;
+      const int gcb = st.group_count[c];
+      for (int fb = 0; fb < gcb; ++fb) {
+        const float* col = hq + st.group_lane[c][fb] * NP;
+        const float mb = st.group_mult[c][fb];
+        for (int fa = 0; fa < gca; ++fa) h = fmaf(mb * st.group_mult[l][fa], col[st.group_lane[l][fa]], h);
       }
-      A[l * (NP + 1) + c] = h;
     }
+    A[l * (NP + 1) + c] = h;
   }
-  // ---- Cholesky of A in place, lane = row, one pivot column per step (fp32, IEEE sqrt and division)
+}
+
+// In-place Cholesky of the [dof][NP+1] row-per-lane matrix A (lane = row, one pivot column per step, fp32, IEEE sqrt and
+// division): the lower factor.  Returns whether a pivot was <= 0 (group-uniform).  Shared by vjp_front and the smoother.
+template <int G>
+__device__ __forceinline__ bool factor_rows(float* A, int dof, int l) {
+  constexpr int NP = G;
   bool bad = false;
   for (int k = 0; k < dof; ++k) {
     __syncwarp();
@@ -1955,6 +1924,75 @@ __device__ __forceinline__ VjpFront vjp_front(Solver<G, 0>& sv, const FrameInput
       for (int j = k + 1; j <= l; ++j) A[l * (NP + 1) + j] = fmaf(-lik, A[j * (NP + 1) + k], A[l * (NP + 1) + j]);
     }
   }
+  return bad;
+}
+
+// What vjp_tail hands back to its driver, per lane: v (H_ff^-1 gbar_f on this lane's variable, 0 elsewhere), the fixed-joint
+// term H_q[c, :] . M v of a fixed lane (its cotangent is -qbar), and the frame's finite / not-positive-definite verdicts
+// (group-uniform).  The keypoint cotangents are in the scratch's kKp accumulator.
+struct VjpLane {
+  float v, qbar;
+  bool finite, bad;
+};
+
+// What vjp_front leaves for vjp_tail besides the scratch (H_q in kH, the factor in kA, the flags in kFlags): whether this
+// lane's variable is free, and the frame's finite / not-positive-definite verdicts (group-uniform).
+struct VjpFront {
+  bool free_, finite, bad;
+};
+
+// The implicit-function VJP of one frame is vjp_front once, then vjp_tail once per cotangent: vjp_frame (dexr_solve_vjp) and
+// vjp_stream (dexr_solve_sequences_vjp) run one tail, jacobian_frame (dexr_solve_jacobian) one per free variable.
+//
+// The per-frame front: the point x, the anchor x0 of this lane's variable come from the driver, with norm_delta `nd`
+// (0: no regulariser) and the frame's DexPilot flags `proj` (read into the scratch; nullptr = all 0); `gbar` only takes
+// part in the finiteness verdict.  Prepares the targets on the private flag copy, runs FK, builds the gradient, the active
+// set and the exact H_q, folds the mimic joints, freezes the active rows and factorises the free block in place in kA.  The
+// caller's flags are never written.
+template <int G>
+__device__ __forceinline__ VjpFront vjp_front(Solver<G, 0>& sv, const FrameInputs& in_, const Dims& dm, float x, float x0,
+                                              float gbar, float nd, const uint8_t* proj, bool active) {
+  using VS = VjpScratch<G>;
+  constexpr int NP = G;
+  const SharedTable& st = Solver<G, 0>::ST();
+  const int l = sv.l, lane = sv.lane, dof = dm.dof;
+  const bool isvar = sv.var >= 0;
+  float* const A = sv.scf() + VS::kA;
+  uint8_t* const flags = reinterpret_cast<uint8_t*>(sv.scf() + VS::kFlags);
+
+  // ---- targets (flags on the private copy), FK at x
+  const int fixedi = st.fixed_index[l];
+  sv.qfix = (active && fixedi >= 0) ? in_.fixed[fixedi] : 0.f;
+  sv.x = x;
+  if (l < dm.len_proj) flags[l] = (active && proj) ? proj[l] : (uint8_t)0;
+  __syncwarp();
+  FrameInputs in = in_;
+  in.projected = dm.len_proj > 0 ? flags : nullptr;
+  bool finite = isfinite(x) && isfinite(x0) && isfinite(sv.qfix) && isfinite(gbar);
+  const bool ok_targets = sv.prepare_targets(in, active);
+  finite = !gany<G>(!finite, lane) && ok_targets;
+  __syncwarp();
+  sv.q = sv.compose_q(x);
+  {
+    float R[9];
+    sv.fk(sv.q, R, sv.p);
+    sv.write_world_links();
+    sv.write_links(R, sv.p, 0);
+    sv.set_world_axis(R);
+  }
+  __syncwarp();
+
+  float g = exact_grad_hq(sv, dm);
+  g = isvar ? fmaf(2.0f * nd, x - x0, g) : 0.f;
+
+  // ---- active set (the solver's rule at its widened bounds), then A = the free block of M^T H_q M + 2 norm_delta I
+  const bool act = isvar && ((x <= sv.lo && g > -kGradNoise) || (x >= sv.hi && g < kGradNoise));
+  const bool free_ = isvar && !act;
+  const unsigned fmask = gballot<G>(free_, lane);
+  __syncwarp();
+  fold_free_block(sv, dm, A, free_, fmask, 2.0f * nd);
+  // ---- Cholesky of A in place
+  const bool bad = factor_rows<G>(A, dof, l);
   __syncwarp();
   return VjpFront{free_, finite, bad};
 }
@@ -2485,6 +2523,339 @@ __device__ __forceinline__ void vjp_packed_stream(Solver<G, 0>& sv, const dexr_s
     if (isvar && io.grad_last_qpos) io.grad_last_qpos[sc * dm.n_var + sv.var] = c;
     if (isjoint && io.grad_filter_state) io.grad_filter_state[sc * dm.dof + l] = gy;
   }
+}
+
+// ------------------------------------------------------------------------------------------------
+// offline smoothing of packed streams (dexr_smooth_sequences_packed): every frame of a stream solved jointly
+// ------------------------------------------------------------------------------------------------
+// F(X) = sum_t L_t(x_t) + w sum_{t>=1} |x_t - x_{t-1}|^2 + w |x_0 - a|^2 is minimised by a damped projected Newton method,
+// one group of G lanes per stream (lane = joint, as in the VJP).  Its Hessian is block tridiagonal: D_t = M^T H_q M + 2 w k_t I
+// (+ mu I, the damping) on the diagonal, -2 w I beside it.  One outer iteration is three sweeps along the clip:
+//   forward   at x_t: targets (the DexPilot flag recurrence), FK, the data gradient and H_q (exact_grad_hq, as in the VJP),
+//             the smoothness gradient, the active set (the solver's rule on the TOTAL gradient), then block Thomas:
+//             S_t = D_t - (2w)^2 Z_{t-1} and y_t = -g_t + 2w Z_{t-1} y_{t-1} over the free variables of frame t, with
+//             Z_t the inverse of S_t over its free variables and zero elsewhere (so the free sets of t-1 and t need no
+//             further masking).  S_t is factorised (factor_rows) and inverted, one column per lane, into the workspace;
+//   backward  delta_t = Z_t (y_t + 2w delta_{t+1}) and the trial clip(x_t + delta_t) to the widened bounds;
+//   cost      sum over frames and lanes of (this lane's term of F_t at the trial) - (the same at x), F_t = L_t(x_t) +
+//             w |x_t - x_{t-1}|^2: per-term differences, not a difference of two fp32 totals over hundreds of frames.
+// A decrease is accepted (mu x 0.1), and so is a change within the fp32 resolution of F when the predicted decrease is
+// too (kSmoothNoise); anything else is rejected (mu x 10).  A pivot <= 0 in the forward sweep restarts it at once, first with
+// the Gauss-Newton model (H_q without the kinematic curvature, positive semi-definite: the positive-definite fallback of the
+// frame solver), then with more damping.  The stream stops when the max |delta| of a trial falls to params.tol, or after
+// params.max_iters accepted outer iterations.
+// A missing frame (non-finite keypoint or fixed joint) keeps only its smoothness terms (H_q = 0, no data gradient).
+//
+// Workspace per frame (floats), lane-space vectors of G entries:
+//   kZ  [G][G] Z_t; entry [k][c] is written and read back by lane c only (column c of the inverse, which lane c uses as its
+//              row: Z_t is symmetric up to rounding), so the accesses are coalesced and never cross lanes
+//   kY  [G]    y_t
+//   kX  [2][G] the iterate and the trial (0 on lanes without a variable)
+//   kV  [G]    this lane's term of F_t at the iterate
+//   kG  [G]    the total gradient g_t on the free variables (0 elsewhere), for the predicted decrease
+template <int G>
+struct SmoothWs {
+  static constexpr int kZ = 0;
+  static constexpr int kY = G * G;
+  static constexpr int kX = kY + G;
+  static constexpr int kV = kX + 2 * G;
+  static constexpr int kG = kV + G;
+  static constexpr int kFloats = kG + G;
+};
+
+// Relative resolution of F in the smoother's acceptance test: a trial whose change of F, and whose predicted decrease
+// -g.delta / 2, both lie within kSmoothNoise F is accepted.  Near the minimiser the decrease a Newton step brings along a
+// flat direction (a joint the keypoints hardly determine) is far below what the fp32 terms resolve; rejecting it there
+// would only raise the damping until the step fell below tol, short of the minimiser.
+constexpr float kSmoothNoise = 1e-6f;
+// Damping beyond which a stream stops (with DEXR_STATUS_MAXITER): its steps are far below any tolerance by then.
+constexpr float kSmoothMuMax = 1e12f;
+
+// Bytes of workspace a call on `num_frames` frames needs (dexr_smooth_workspace_bytes).
+inline size_t smooth_workspace_bytes(const dexr_table_t& t, long long num_frames) {
+  const int floats = eval_lanes(t) == 16 ? SmoothWs<16>::kFloats : SmoothWs<32>::kFloats;
+  return num_frames > 0 ? (size_t)num_frames * (size_t)floats * sizeof(float) : 0;
+}
+
+// The argument checks of dexr_smooth_sequences_packed: nullptr, or what is wrong.  Host code shared by the library and the
+// host emulation.  offsets live on the device and are not read here.
+inline const char* smooth_io_error(const dexr_table_t& t, const dexr_smooth_t& io, const dexr_params_t& prm,
+                                   const int64_t* offsets, long long S, long long N) {
+  if (S < 0 || N < 0 || N > INT32_MAX) return "bad sizes: num_streams and num_frames must be >= 0, num_frames <= INT32_MAX";
+  if (!offsets) return "offsets (device [S+1]) are required";
+  if (prm.preprocess != 0) return "raw landmarks are not smoothed: params.preprocess must be 0 (pre-process the keypoints first)";
+  if (!io.keypoints || !io.qpos_init || !io.qpos_out) return "keypoints, qpos_init and qpos_out are required";
+  if (t.n_fixed > 0 && !io.fixed_qpos) return "the robot has fixed joints but fixed_qpos is NULL";
+  if (!(io.smooth_weight < 0.f) && !(io.smooth_weight >= 0.f && io.smooth_weight <= 3.0e38f))
+    return "smooth_weight must be finite (< 0: params.norm_delta)";
+  if (N > 0 && (!io.workspace || io.workspace_bytes < smooth_workspace_bytes(t, N)))
+    return "workspace smaller than dexr_smooth_workspace_bytes(robot, num_frames)";
+  return nullptr;
+}
+
+// Whether frame fr has a non-finite keypoint coordinate or fixed joint (group-uniform; false for a group that is not `live`).
+template <int G>
+__device__ __forceinline__ bool smooth_missing(const Solver<G, 0>& sv, const dexr_smooth_t& io, const Dims& dm, long long fr,
+                                               bool live) {
+  bool bad = false;
+  if (live) {
+    const float* kp = io.keypoints + fr * (3 * DEXR_NUM_KEYPOINTS);
+    for (int e = sv.l; e < 3 * DEXR_NUM_KEYPOINTS; e += G) bad = bad || !isfinite(kp[e]);
+    const int fixedi = Solver<G, 0>::ST().fixed_index[sv.l];
+    if (fixedi >= 0) bad = bad || !isfinite(io.fixed_qpos[fr * dm.n_fixed + fixedi]);
+  }
+  return gany<G>(bad, sv.lane);
+}
+
+// Frame fr at the point x (this lane's variable; xp: the previous frame's, or the anchor, when `has_prev`): advances the
+// group's DexPilot flags in the scratch by one step of the hysteresis recurrence, prepares the targets, runs FK and returns
+// this lane's term of F_t -- residual l of L_t (none for a missing frame) plus w (x - xp)^2 on a variable lane (w is
+// sv.prm.norm_delta, which the launch sets to the smoothing weight).
+template <int G>
+__device__ __forceinline__ float smooth_eval(Solver<G, 0>& sv, const dexr_smooth_t& io, const Dims& dm, long long fr, float x,
+                                             float xp, bool has_prev, bool missing, bool live) {
+  const int l = sv.l;
+  const int fixedi = Solver<G, 0>::ST().fixed_index[l];
+  const float qf = (live && fixedi >= 0) ? io.fixed_qpos[fr * dm.n_fixed + fixedi] : 0.f;
+  sv.qfix = isfinite(qf) ? qf : 0.f;
+  sv.x = x;
+  sv.x0 = has_prev ? xp : x;
+  FrameInputs in;
+  in.kp = io.keypoints + fr * (3 * DEXR_NUM_KEYPOINTS);
+  in.ref = nullptr;
+  in.fixed = nullptr;
+  in.last = nullptr;
+  in.projected = dm.len_proj > 0 ? reinterpret_cast<uint8_t*>(sv.scf() + VjpScratch<G>::kFlags) : nullptr;
+  sv.prepare_targets(in, live);
+  __syncwarp();
+  sv.q = sv.compose_q(x);
+  {
+    float R[9];
+    sv.fk(sv.q, R, sv.p);
+    sv.write_world_links();
+    sv.write_links(R, sv.p, 0);
+    sv.set_world_axis(R);
+  }
+  __syncwarp();
+  sv.cost(0, x);
+  const float dx = x - sv.x0;
+  const float reg = sv.var >= 0 ? fmaf(sv.prm.norm_delta * dx, dx, 0.f) : 0.f;
+  return missing ? reg : sv.cost_lane;
+}
+
+// The group's DexPilot flags at the start of stream sc (nullptr: all false), into the scratch copy the sweeps advance.
+template <int G>
+__device__ __forceinline__ void smooth_reset_flags(const Solver<G, 0>& sv, const dexr_smooth_t& io, const Dims& dm, long long sc,
+                                                   bool has) {
+  uint8_t* const flags = reinterpret_cast<uint8_t*>(sv.scf() + VjpScratch<G>::kFlags);
+  if (sv.l < dm.len_proj) flags[sv.l] = (has && io.projected) ? io.projected[sc * dm.len_proj + sv.l] : (uint8_t)0;
+  __syncwarp();
+}
+
+// One packed stream `ps` (ps.s < 0: none) of dexr_smooth_sequences_packed; `owner`: this group runs the stream (the kernel
+// gives a 16-lane warp's second group none).  The warp walks its groups' longer stream in every sweep and iterates until
+// every group is done; a group that is done, or past its stream's end, runs its frames inactive with its writes off.  `ws`: the workspace,
+// SmoothWs<G>::kFloats per frame.  `dm` and `prm` are the kernel argument's.
+template <int G>
+__device__ __forceinline__ void smooth_packed_stream(Solver<G, 0>& sv, const dexr_smooth_t& io, const Dims& dm,
+                                                     const dexr_params_t& prm, const PackedStream& ps, bool owner, float* ws) {
+  using W = SmoothWs<G>;
+  constexpr int NP = G;
+  const SharedTable& st = Solver<G, 0>::ST();
+  const int l = sv.l, lane = sv.lane, dof = dm.dof, n = dm.n_var;
+  const bool isvar = sv.var >= 0;
+  const bool valid = owner && ps.s >= 0;
+  const int len = valid ? ps.len : 0;
+  const int steps = warp_steps<G>(len);
+  if (steps == 0) return;
+  const bool has = len > 0;
+  const long long sc = has ? ps.s : 0, f0 = has ? ps.first : 0;
+  const int tlast = has ? len - 1 : 0;
+  float* const wsf = ws + f0 * W::kFloats;
+  float* const A = sv.scf() + VjpScratch<G>::kA;
+  float* const hq = sv.scf() + VjpScratch<G>::kH;
+  const float w = sv.prm.norm_delta, w2 = 2.0f * w;
+  const bool anchor = io.last_qpos != nullptr;
+
+  // ---- the anchor and the starting trajectory (clipped to the widened bounds), both checked for finiteness
+  bool nonfinite = false;
+  float a = 0.f;
+  if (has && isvar && anchor) {
+    const float ar = io.last_qpos[sc * n + sv.var];
+    nonfinite = !isfinite(ar);
+    a = fminf(fmaxf(ar, st.clip_lo[l]), st.clip_hi[l]);
+  }
+  for (int t = 0; t < len; ++t) {
+    float x = 0.f;
+    if (isvar) {
+      const float v = io.qpos_init[(f0 + t) * n + sv.var];
+      nonfinite = nonfinite || !isfinite(v);
+      x = fminf(fmaxf(v, sv.lo), sv.hi);
+    }
+    wsf[t * W::kFloats + W::kX + l] = x;
+  }
+  nonfinite = gany<G>(nonfinite, lane);
+
+  // ---- outer iterations (every counter and verdict below is group-uniform).  `exact`: the forward sweep uses the exact
+  // Hessians; after an elimination that met a pivot <= 0 the sweep is repeated at the same damping with the Gauss-Newton
+  // model (positive semi-definite, so the system is positive definite), then with ten times the damping.
+  float mu = prm.lambda0, F = 0.f;
+  int cur = 0, iters = 0, rejects = 0;
+  bool done = !has || nonfinite, maxit = false, exact = true;
+  while (__ballot_sync(0xffffffffu, !done) != 0u) {
+    const bool act = !done;
+    // forward sweep
+    smooth_reset_flags(sv, io, dm, sc, has);
+    bool failed = false;
+    float fsum = 0.f, yprev = 0.f;
+    for (int t = 0; t < steps; ++t) {
+      const bool live = act && t < len;
+      const int tc = t < tlast ? t : tlast;
+      const long long fr = f0 + tc;
+      float* const wt = wsf + tc * W::kFloats;
+      const bool missing = smooth_missing(sv, io, dm, fr, live);
+      const bool has_prev = t > 0 || anchor, has_next = t + 1 < len;
+      // (frame tc of the group's stream, or frame 0 without one, is in the workspace; its neighbours only while `live`)
+      const float x = wt[W::kX + cur * G + l];
+      const float xp = (live && t > 0) ? wt[W::kX + cur * G + l - W::kFloats] : a;
+      const float xn = (live && has_next) ? wt[W::kX + cur * G + l + W::kFloats] : 0.f;
+      const float v = smooth_eval(sv, io, dm, fr, x, xp, has_prev, missing, live);
+      if (live) {
+        wt[W::kV + l] = v;
+        fsum += v;
+      }
+      float g = exact_grad_hq(sv, dm, exact);
+      if (missing) {
+        g = 0.f;
+#pragma unroll
+        for (int i = 0; i < NP; ++i) hq[i * NP + l] = 0.f;
+      }
+      g = isvar ? g + (has_prev ? w2 * (x - xp) : 0.f) + (has_next ? w2 * (x - xn) : 0.f) : 0.f;
+      const bool at_bound = isvar && ((x <= sv.lo && g > -kGradNoise) || (x >= sv.hi && g < kGradNoise));
+      const bool free_ = live && isvar && !at_bound;
+      const unsigned fmask = gballot<G>(free_, lane);
+      __syncwarp();
+      fold_free_block(sv, dm, A, free_, fmask, fmaf(w2, (float)((has_prev ? 1 : 0) + (has_next ? 1 : 0)), mu));
+      float y = free_ ? -g : 0.f;
+      if (t > 0) {  // (warp-uniform) the Schur complement of frame t - 1: Z_{t-1} is zero off its free variables
+        const float* zp = wt - W::kFloats + W::kZ;
+        float zy = 0.f;
+        for (int c = 0; c < dof; ++c) {
+          const float z = live ? zp[c * G + l] : 0.f;
+          zy = fmaf(z, gshfl<G>(yprev, c), zy);
+          if (free_ && ((fmask >> c) & 1u)) A[l * (NP + 1) + c] = fmaf(-w2 * w2, z, A[l * (NP + 1) + c]);
+        }
+        if (free_) y = fmaf(w2, zy, y);
+      }
+      const bool bad = factor_rows<G>(A, dof, l);
+      __syncwarp();
+      failed = failed || (live && bad);
+      // Z_t, column l: L L^T z = e_l by forward and back substitution over the factor, z in the kH area (H_q is folded
+      // into A by now), entry k of lane l at hq[k * NP + l]: the factor's reads are broadcasts, z's conflict-free
+      for (int k = 0; k < dof; ++k) {
+        float s = k == l ? 1.0f : 0.f;
+        for (int i = 0; i < k; ++i) s = fmaf(-A[k * (NP + 1) + i], hq[i * NP + l], s);
+        hq[k * NP + l] = s / A[k * (NP + 1) + k];
+      }
+      for (int k = dof - 1; k >= 0; --k) {
+        float s = hq[k * NP + l];
+        for (int i = k + 1; i < dof; ++i) s = fmaf(-A[i * (NP + 1) + k], hq[i * NP + l], s);
+        s = s / A[k * (NP + 1) + k];
+        hq[k * NP + l] = s;
+        if (live) wt[W::kZ + k * G + l] = (free_ && ((fmask >> k) & 1u)) ? s : 0.f;
+      }
+      if (live) {
+        wt[W::kY + l] = y;
+        wt[W::kG + l] = free_ ? g : 0.f;
+      }
+      yprev = y;
+      __syncwarp();  // the next frame rewrites the scratch this one read
+    }
+    const float Fold = gsum<G>(fsum);
+    if (act) F = Fold;
+    const bool go = act && !failed;
+    if (act && failed) {  // restart the forward sweep: no trial, no outer iteration
+      if (exact) exact = false;
+      else mu *= kLamUp;
+      if (rejects < 127) ++rejects;
+      if (!(mu <= kSmoothMuMax)) done = maxit = true;
+    }
+    if (__ballot_sync(0xffffffffu, go) == 0u) continue;  // (warp-uniform) no group has a trial to evaluate
+    // backward sweep: the step and the trial
+    float dn = 0.f, smax = 0.f, gd = 0.f;
+    for (int t = steps - 1; t >= 0; --t) {
+      const bool live = go && t < len;
+      const int tc = t < tlast ? t : tlast;
+      float* const wt = wsf + tc * W::kFloats;
+      const float r = live ? wt[W::kY + l] + (t + 1 < len ? w2 * dn : 0.f) : 0.f;
+      float d = 0.f;
+      for (int c = 0; c < dof; ++c) d = fmaf(live ? wt[W::kZ + c * G + l] : 0.f, gshfl<G>(r, c), d);
+      if (live) {
+        const float x = wt[W::kX + cur * G + l];
+        wt[W::kX + (cur ^ 1) * G + l] = isvar ? fminf(fmaxf(x + d, sv.lo), sv.hi) : 0.f;
+        smax = fmaxf(smax, fabsf(d));
+        gd = fmaf(wt[W::kG + l], d, gd);
+        dn = d;
+      }
+    }
+    smax = gmax<G>(smax);
+    const float pred = -0.5f * gsum<G>(gd);
+    // cost sweep: per-term differences of F_t at the trial and at x
+    smooth_reset_flags(sv, io, dm, sc, has);
+    float dsum = 0.f, fnew = 0.f;
+    for (int t = 0; t < steps; ++t) {
+      const bool live = go && t < len;
+      const int tc = t < tlast ? t : tlast;
+      const long long fr = f0 + tc;
+      float* const wt = wsf + tc * W::kFloats;
+      const bool missing = smooth_missing(sv, io, dm, fr, live);
+      const float x = wt[W::kX + (cur ^ 1) * G + l];
+      const float xp = (live && t > 0) ? wt[W::kX + (cur ^ 1) * G + l - W::kFloats] : a;
+      const float v = smooth_eval(sv, io, dm, fr, x, xp, t > 0 || anchor, missing, live);
+      if (live) {
+        dsum += v - wt[W::kV + l];
+        fnew += v;
+      }
+      __syncwarp();
+    }
+    const float dF = gsum<G>(dsum), Fnew = gsum<G>(fnew);
+    if (go) {
+      if (dF < 0.f || (dF <= kSmoothNoise * Fold && pred <= kSmoothNoise * Fold)) {
+        cur ^= 1;
+        ++iters;
+        mu = fmaxf(mu * kLamDown, kLamMin);
+        F = Fnew;
+      } else {
+        mu *= kLamUp;
+        if (rejects < 127) ++rejects;
+      }
+      exact = true;
+      done = smax <= prm.tol;
+      if (!done && (iters >= prm.max_iters || !(mu <= kSmoothMuMax))) done = maxit = true;
+    }
+  }
+
+  // ---- outputs: the answer (qpos_init as given for a non-finite start), its scatter + mimic, the status, the cost
+  const int base_status = nonfinite ? DEXR_STATUS_NONFINITE
+                                    : ((iters & 0xffff) | (rejects << 16) | (maxit ? DEXR_STATUS_MAXITER : 0));
+  const int fixedi = st.fixed_index[l];
+  for (int t = 0; t < steps; ++t) {
+    const bool live = has && t < len;
+    const int tc = t < tlast ? t : tlast;
+    const long long fr = f0 + tc;
+    const bool missing = smooth_missing(sv, io, dm, fr, live && !nonfinite);
+    float x = 0.f;
+    if (live && isvar) x = nonfinite ? io.qpos_init[fr * n + sv.var] : wsf[tc * W::kFloats + W::kX + cur * G + l];
+    sv.qfix = (live && fixedi >= 0) ? io.fixed_qpos[fr * dm.n_fixed + fixedi] : 0.f;
+    const float q = sv.compose_q(x);
+    if (live) {
+      if (isvar) io.qpos_out[fr * n + sv.var] = x;
+      if (io.robot_qpos_out && l < dof) io.robot_qpos_out[fr * dof + l] = q;
+      if (io.status_out && l == 0) io.status_out[fr] = base_status | (missing ? DEXR_STATUS_MISSING : 0);
+    }
+  }
+  if (has && io.cost_out && l == 0) io.cost_out[sc] = nonfinite ? __int_as_float(0x7fc00000) : F;
+  __syncwarp();
 }
 
 }  // namespace dexr

@@ -13,6 +13,8 @@ With a `SequenceTape` the same launch also records every frame's unfiltered solu
 (`dexr_solve_sequences_vjp`; `objective.differentiable_retarget_sequences` wraps both for autograd).
 `retarget_packed_sequences()` / `retarget_packed_sequences_vjp()` do the same for streams of different lengths laid end to
 end (`PackedStreams`, the cu_seqlens layout): recorded clips of any length in one launch, no padding.
+`smooth_packed_sequences()` solves every frame of each packed clip jointly (`dexr_smooth_sequences_packed`): the offline
+trajectory, with no lag and with dropped frames filled in.
 """
 from __future__ import annotations
 
@@ -584,3 +586,62 @@ class SeqRetargeting:
                                                         C.c_void_p(s.cuda_stream)),
                 "dexr_solve_sequences_packed_vjp")
         return g_kp, g_fixed, g_last, g_filter
+
+    def smooth_packed_sequences(self, keypoints, layout: PackedStreams, state: Optional[StreamState] = None, *,
+                                fixed_qpos=None, qpos_init=None, smooth_weight=None, out=None, status_out=None, stream=None):
+        """Offline smoothing of recorded clips (`dexr_smooth_sequences_packed`, one launch): every frame of each packed
+        stream solved jointly, minimising sum_t L_t(x_t) + w sum_t |x_t - x_{t-1}|^2 + w |x_0 - clip(a)|^2 over the
+        clip.  With w = norm_delta (`smooth_weight` None) this is the sum of the costs `retarget_packed_sequences` minimises
+        one frame at a time, without its lag.  keypoints [N,21,3] (wrist-centred, not raw landmarks) and fixed_qpos
+        [N,n_fixed] as for `retarget_packed_sequences`; `state` is read only: the anchor a is `state.last_qpos` and the
+        DexPilot flags start at `state.projected` (None: a fresh `make_stream_state`).  `qpos_init` [N,opt_dof] is the
+        starting trajectory; None runs the taped `retarget_packed_sequences` on a copy of the state and starts from its
+        tape.  A frame with a non-finite keypoint or fixed joint is filled in by the smoothness terms (STATUS_MISSING).
+        Returns (robot_qpos [N,dof] (scatter + mimic, no low-pass filter), qpos [N,opt_dof], status [N] int32); a stream
+        whose status has STATUS_MAXITER returns its last accepted iterate (lower F than its start), not the minimiser.  Allocates
+        its workspace on the device; nothing is synchronised."""
+        import torch
+
+        opt = self.optimizer
+        eng = opt.engine()
+        dev = torch.device("cuda", eng.device)
+        S, N_ = layout.num_streams, layout.num_frames
+        n, dof, nf = opt.opt_dof, opt.robot.dof, len(opt.idx_pin2fixed)
+        chk = _checker(dev)
+        if state is None:
+            state = self.make_stream_state(S)
+        io = N.DexrSmooth()
+        io.keypoints = chk(keypoints, (N_, N.NUM_KEYPOINTS, 3), torch.float32, "keypoints")
+        if nf:
+            if fixed_qpos is None:
+                raise ValueError(f"Optimizer has {nf} fixed joints but no fixed_qpos is given")
+            io.fixed_qpos = chk(fixed_qpos, (N_, nf), torch.float32, "fixed_qpos")
+        io.last_qpos = chk(state.last_qpos, (S, n), torch.float32, "state.last_qpos")
+        if state.projected is not None:
+            io.projected = chk(state.projected, (S, state.projected.shape[1]), torch.uint8, "state.projected")
+        offsets = chk(layout.offsets, (S + 1,), torch.int64, "layout.offsets")
+        if qpos_init is None:
+            tape = self.make_packed_sequence_tape(layout)
+            copy = StreamState(**{k: (None if getattr(state, k) is None else getattr(state, k).clone())
+                                  for k in StreamState._FIELDS})
+            self.retarget_packed_sequences(keypoints, layout, copy, fixed_qpos=fixed_qpos, stream=stream, tape=tape)
+            qpos_init = tape.qpos
+        io.qpos_init = chk(qpos_init, (N_, n), torch.float32, "qpos_init")
+        qpos = torch.empty((N_, n), dtype=torch.float32, device=dev)
+        io.qpos_out = qpos.data_ptr()
+        if out is None:
+            out = torch.empty((N_, dof), dtype=torch.float32, device=dev)
+        io.robot_qpos_out = chk(out, (N_, dof), torch.float32, "out")
+        if status_out is None:
+            status_out = torch.empty((N_,), dtype=torch.int32, device=dev)
+        io.status_out = chk(status_out, (N_,), torch.int32, "status_out")
+        io.smooth_weight = -1.0 if smooth_weight is None else float(smooth_weight)
+        nbytes = int(eng.lib.dexr_smooth_workspace_bytes(eng.handle, N_))
+        ws = torch.empty((max(nbytes, 4),), dtype=torch.uint8, device=dev)
+        io.workspace, io.workspace_bytes = ws.data_ptr(), nbytes
+        s = stream if stream is not None else torch.cuda.current_stream(dev)
+        p = opt.params(clip_init=True, lp_alpha=self.low_pass_alpha)
+        N.check(eng.lib.dexr_smooth_sequences_packed(eng.handle, C.byref(p), C.byref(io), C.c_void_p(offsets), S, N_,
+                                                     C.c_void_p(s.cuda_stream)), "dexr_smooth_sequences_packed")
+        ws.record_stream(s)
+        return out, qpos, status_out

@@ -414,6 +414,57 @@ int dexr_solve_sequences_packed(const dexr_robot_t* robot, const dexr_params_t* 
 int dexr_solve_sequences_packed_vjp(const dexr_robot_t* robot, const dexr_params_t* params, const dexr_sequences_vjp_t* io,
                                     const int64_t* offsets, int64_t num_streams, int64_t num_frames, void* cuda_stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Offline trajectory smoothing of packed streams: every frame of a stream solved JOINTLY.  Per stream of T frames,
+ *   F(X) = sum_t L_t(x_t) + w sum_{t>=1} |x_t - x_{t-1}|^2 + w |x_0 - clip(a)|^2,   x_t in [lower, upper] (widened bounds)
+ * with L_t the per-frame loss of the solve (position / vector / DexPilot, mimic and fixed joints), a the stream's warm start
+ * (last_qpos; NULL: no anchor term) clipped to clip_lo / clip_hi, and w = smooth_weight (< 0: params.norm_delta).  With
+ * w = norm_delta, F is the sum of the costs the causal solve (dexr_solve_sequences_packed) minimises one frame at a time;
+ * the joint minimiser has no lag.  One group of lanes per stream runs a damped projected Newton method on F: the Hessian is
+ * block tridiagonal (diagonal blocks the exact per-frame Hessians + 2 w k_t I, k_t the frame's neighbours with the anchor
+ * counting as one; off-diagonal blocks -2 w I), eliminated along the clip by block Thomas.
+ *   Layout: packed only, with the offsets and malformed-range rules of dexr_solve_sequences_packed (an equal-length batch is
+ *     the rectangular layout); keypoints, fixed_qpos, qpos_init, qpos_out, robot_qpos_out, status_out [N,...];
+ *     last_qpos, projected, cost_out [S,...].  A stream of length 0 writes nothing.
+ *   DexPilot: frame t uses the flags the causal packed solve leaves at frame t -- the hysteresis recurrence, which reads only
+ *     the human vectors, walked along the clip from projected[s].  The flags are not optimised; projected is never written.
+ *   Missing frames: a frame with a non-finite keypoint coordinate or fixed joint has no data term and gets
+ *     DEXR_STATUS_MISSING; its output is what the smoothness terms give: an interior gap the linear interpolation (in
+ *     variable space) of the frames on either side, a trailing gap the last observed frame, a leading gap the
+ *     interpolation from the clipped anchor (the first observed frame repeated when there is no anchor).
+ *   Non-finite start: a stream whose qpos_init (or anchor, when given) is non-finite gets qpos_init back, every frame of it
+ *     DEXR_STATUS_NONFINITE and cost NaN; no other stream changes.
+ *   Status: the low 16 bits hold the stream's accepted outer iterations and bits 16-22 its rejected trials and restarted
+ *     eliminations (saturating at 127), on every frame of the stream; DEXR_STATUS_MAXITER after params.max_iters accepted
+ *     outer iterations.  params.tol is the stopping step (max |delta| over the stream), params.lambda0 the initial damping
+ *     (x 0.1 after an accepted step, x 10 after a rejected one).  An elimination that meets a pivot <= 0 (an indefinite
+ *     exact Hessian) is restarted with the Gauss-Newton model, then with more damping; it uses up no outer iteration.
+ *   The starting trajectory is clipped to the widened bounds.  Raw landmarks (params.preprocess != 0) are refused.
+ *   `workspace`: device scratch of at least dexr_smooth_workspace_bytes(robot, num_frames) bytes (DEXR_E_INVALID below);
+ *   the call allocates nothing and never synchronises.  All pointers are DEVICE pointers.
+ * ------------------------------------------------------------------------------------------- */
+#define DEXR_STATUS_MISSING (1 << 27) /* smoother: the frame's inputs were non-finite; its output is interpolated by the
+                                         smoothness terms alone (informational, not a failure) */
+typedef struct dexr_smooth {
+  const float* keypoints;   /* [N,21,3] wrist-centred MANO keypoints (params.preprocess must be 0)                   */
+  const float* fixed_qpos;  /* [N,n_fixed] or NULL when n_fixed == 0                                                   */
+  const float* last_qpos;   /* [S,n_var] warm start a of each stream (clipped to clip_lo/clip_hi), or NULL: no anchor term */
+  const uint8_t* projected; /* [S,len_proj] DexPilot flags at the start of each stream, read only (NULL: all false)   */
+  const float* qpos_init;   /* [N,n_var] starting trajectory, normally the tape of dexr_solve_sequences_packed           */
+  float* qpos_out;          /* [N,n_var] the answer (may equal qpos_init): the minimiser unless DEXR_STATUS_MAXITER    */
+  float* robot_qpos_out;    /* [N,dof] or NULL: scatter + mimic of qpos_out, NO low-pass filter                        */
+  int32_t* status_out;      /* [N] or NULL                                                                              */
+  float* cost_out;          /* [S] or NULL: F at the answer                                                             */
+  float smooth_weight;      /* w; < 0: params.norm_delta                                                                */
+  void* workspace;          /* device scratch of at least dexr_smooth_workspace_bytes(robot, num_frames) bytes          */
+  size_t workspace_bytes;
+} dexr_smooth_t;
+size_t dexr_smooth_sizeof(void);
+size_t dexr_smooth_workspace_bytes(const dexr_robot_t* robot, int64_t num_frames);
+int dexr_smooth_sequences_packed(const dexr_robot_t* robot, const dexr_params_t* params, const dexr_smooth_t* io,
+                                 const int64_t* offsets /* device [S+1] */, int64_t num_streams, int64_t num_frames,
+                                 void* cuda_stream);
+
 #ifdef __cplusplus
 }
 #endif
