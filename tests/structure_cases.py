@@ -98,16 +98,17 @@ def solver_kind(t, use_arrow=True):
     return "<32,-1>" if t.arrow > 0 and use_arrow else "<32,0>"
 
 
-def build(case, tmp_path):
-    """(SeqRetargeting of the product, OracleOptimizer) for the case, with the table checked against its features."""
+def build(case, tmp_path, override=None):
+    """(SeqRetargeting of the product, OracleOptimizer) for the case, with the table checked against its features.
+    `override`: configuration entries to change (as for helpers.build_product), e.g. {"low_pass_alpha": -1.0}."""
     from dex_retargeting_b200.retargeting_config import RetargetingConfig
     from oracle.objectives import OracleOptimizer
 
     d = tmp_path / case.id
     d.mkdir(parents=True, exist_ok=True)
     _, cfg = write_tree_hand(d, case.trunk, case.widths, kind=case.kind, name=case.id, **case.opts)
-    seq = RetargetingConfig.from_dict(dict(cfg)).build()
-    o = OracleOptimizer(dict(cfg), str(d))
+    seq = RetargetingConfig.from_dict(dict(cfg), override).build()
+    o = OracleOptimizer(dict(cfg), str(d), override)
     assert o.robot.dof_joint_names == seq.optimizer.robot.dof_joint_names
     check_features(case, seq.optimizer.build_table())
     return seq, o
