@@ -127,6 +127,18 @@ class DexrSmooth(C.Structure):
     ]
 
 
+class DexrSmoothVjp(C.Structure):
+    """Mirror of `dexr_smooth_vjp_t`: buffers of one backpropagation through the smoother
+    (`dexr_smooth_sequences_packed_vjp`)."""
+
+    _fields_ = [
+        ("keypoints", C.c_void_p), ("fixed_qpos", C.c_void_p), ("last_qpos", C.c_void_p), ("projected", C.c_void_p),
+        ("qpos", C.c_void_p), ("grad_qpos", C.c_void_p), ("grad_robot_qpos", C.c_void_p), ("smooth_weight", _f),
+        ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t), ("grad_keypoints", C.c_void_p),
+        ("grad_fixed_qpos", C.c_void_p), ("grad_last_qpos", C.c_void_p), ("status_out", C.c_void_p),
+    ]
+
+
 class DexrGroup(C.Structure):
     """Mirror of `dexr_group_t`: one (robot, batch) group of a mixed-robot launch."""
 
@@ -149,7 +161,8 @@ EXPORTS = [
     "dexr_preprocess_keypoints", "dexr_eval_sizeof", "dexr_eval_objective", "dexr_vjp_sizeof", "dexr_solve_vjp",
     "dexr_sequences_tape_sizeof", "dexr_solve_sequences_tape", "dexr_sequences_vjp_sizeof", "dexr_solve_sequences_vjp",
     "dexr_jacobian_sizeof", "dexr_solve_jacobian", "dexr_solve_sequences_packed", "dexr_solve_sequences_packed_vjp",
-    "dexr_smooth_sizeof", "dexr_smooth_workspace_bytes", "dexr_smooth_sequences_packed",
+    "dexr_smooth_sizeof", "dexr_smooth_workspace_bytes", "dexr_smooth_sequences_packed", "dexr_smooth_vjp_sizeof",
+    "dexr_smooth_sequences_packed_vjp",
 ]
 
 _LIB = None
@@ -262,6 +275,15 @@ def load():
                                                      C.c_int64, C.c_int64, C.c_void_p]
     elif not os.environ.get("DEXR_LIBRARY"):
         raise DexrError(f"{path} does not export dexr_smooth_sizeof: rebuild it (python -m dex_retargeting_b200.build --force)")
+    if hasattr(lib, "dexr_smooth_vjp_sizeof"):
+        lib.dexr_smooth_vjp_sizeof.restype = C.c_size_t
+        if lib.dexr_smooth_vjp_sizeof() != C.sizeof(DexrSmoothVjp):
+            raise DexrError("dexr_smooth_vjp_t layout mismatch between library and binding (stale DEXR_LIBRARY?)")
+        lib.dexr_smooth_sequences_packed_vjp.argtypes = [C.c_void_p, C.POINTER(DexrParams), C.POINTER(DexrSmoothVjp),
+                                                         C.c_void_p, C.c_int64, C.c_int64, C.c_void_p]
+    elif not os.environ.get("DEXR_LIBRARY"):
+        raise DexrError(f"{path} does not export dexr_smooth_vjp_sizeof: rebuild it "
+                        "(python -m dex_retargeting_b200.build --force)")
     # (an older A/B library named by DEXR_LIBRARY reads a prefix of the buffer structs -- fields are only ever appended -- so
     # the single-robot entry points still work with it; dexr_solve_frames_multi, whose groups embed the struct, does not)
     _LIB = lib

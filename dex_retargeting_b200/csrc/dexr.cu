@@ -517,6 +517,32 @@ __global__ void __launch_bounds__(kEvalWarps * 32, G == 16 ? 2 : 1) dexr_smooth_
   }
 }
 
+// backpropagation through the smoother: dexr_smooth_kernel's launch shape, stream slots and workspace
+struct SmoothVjpArgs {
+  const dexr_table_t* table;
+  dexr_params_t prm;  // norm_delta holds the smoothing weight w
+  dexr_smooth_vjp_t io;
+  long long S;
+  Dims dm;
+  int scratch_off;
+};
+
+template <int G>
+__global__ void __launch_bounds__(kEvalWarps * 32, G == 16 ? 2 : 1) dexr_smooth_vjp_kernel(const SmoothVjpArgs a,
+                                                                                           const PackedLayout pk) {
+  load_shared_table(*reinterpret_cast<SharedTable*>(dsmem), a.table);
+  __syncthreads();
+  constexpr int GPW = 32 / G;
+  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
+  const int lane = threadIdx.x & 31;
+  const int gid = warp * GPW + lane / G;
+  Solver<G, 0> sv;
+  sv.init(a.table, a.dm, (uint32_t)(a.scratch_off + gid * VjpScratch<G>::kFloats * 4), a.prm, lane);
+  // (one 64-bit stream index live across the stream, not a base and an offset: the 16-lane kernel has 128 registers)
+  for (long long i = (long long)warp * gridDim.x + blockIdx.x; i < a.S; i += (long long)gridDim.x * kEvalWarps)
+    smooth_vjp_packed_stream(sv, a.io, a.dm, pk, i, lane < G);
+}
+
 // ------------------------------------------------------------------------------------------------
 // keypoint pre-processing (single_hand_detector.py:100-103, 130-158): one thread per frame for the 3x3 frame,
 // tile staged through shared memory so that global loads / stores are coalesced 16-byte accesses
@@ -1558,6 +1584,53 @@ extern "C" int dexr_smooth_sequences_packed(const dexr_robot_t* robot, const dex
   cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
   const PackedLayout pk{offsets, num_streams, num_frames};
   return eval_lanes(r->host) == 16 ? launch_smooth<16>(r, params, io, pk, stream) : launch_smooth<32>(r, params, io, pk, stream);
+}
+
+// dexr_smooth_sequences_packed_vjp: launch_smooth's CTA and occupancy rule.
+template <int G>
+static int launch_smooth_vjp(dexr_robot* r, const dexr_params_t* prm, const dexr_smooth_vjp_t* io, const PackedLayout& pk,
+                             cudaStream_t stream) {
+  SmoothVjpArgs a{};
+  a.table = r->table_dev;
+  a.prm = *prm;
+  if (!(io->smooth_weight < 0.f)) a.prm.norm_delta = io->smooth_weight;
+  a.io = *io;
+  a.S = pk.S;
+  a.dm = make_dims(r->host);
+  a.scratch_off = round_up((int)sizeof(SharedTable), 16);
+  constexpr int GPW = 32 / G;
+  const int smem = a.scratch_off + kEvalWarps * GPW * VjpScratch<G>::kFloats * 4;
+  auto kern = dexr_smooth_vjp_kernel<G>;
+  CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  int per_sm = 1;
+  if (int e = eval_ctas_per_sm(kern, smem, &per_sm)) return e;
+  const long long ctas = pk.S;
+  const int grid = (int)std::min<long long>(ctas, (long long)r->num_sms * per_sm);
+  kern<<<grid, kEvalWarps * 32, smem, stream>>>(a, pk);
+  CUDA_TRY(cudaGetLastError());
+  {
+    std::lock_guard<std::mutex> lk(r->info_mu);
+    r->last = dexr_launch_info_t{grid, kEvalWarps * 32, smem, 0, G, kEvalWarps, r->last.kernels_launched + 1};
+  }
+  return 0;
+}
+
+extern "C" size_t dexr_smooth_vjp_sizeof(void) { return sizeof(dexr_smooth_vjp_t); }
+
+extern "C" int dexr_smooth_sequences_packed_vjp(const dexr_robot_t* robot, const dexr_params_t* params,
+                                                const dexr_smooth_vjp_t* io, const int64_t* offsets, int64_t num_streams,
+                                                int64_t num_frames, void* cuda_stream) {
+  if (!robot || !params || !io) return fail(DEXR_E_INVALID, "dexr_smooth_sequences_packed_vjp: null argument");
+  if (const char* msg = smooth_vjp_io_error(robot->host, *io, *params, offsets, num_streams, num_frames))
+    return fail(DEXR_E_INVALID, "%s", msg);
+  if (int e = check_loss_params(params)) return e;
+  if (num_streams == 0 || num_frames == 0) return 0;
+  DEVICE_SCOPE(robot->device);
+  dexr_robot* r = const_cast<dexr_robot*>(robot);
+  cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
+  const PackedLayout pk{offsets, num_streams, num_frames};
+  return eval_lanes(r->host) == 16 ? launch_smooth_vjp<16>(r, params, io, pk, stream)
+                                   : launch_smooth_vjp<32>(r, params, io, pk, stream);
 }
 
 extern "C" {

@@ -2002,7 +2002,9 @@ __device__ __forceinline__ VjpFront vjp_front(Solver<G, 0>& sv, const FrameInput
 // target pass -- the ref_value cotangents go to `grad_ref` ([m,3] of the frame, or nullptr), the keypoint ones to the kKp
 // accumulator, which it clears first -- and forms the fixed-joint term; everything but grad_ref goes back to the driver.
 // Reads the scratch the front left and writes only kMv and kKp, so it can run any number of times after one front.
-template <int G>
+// SOLVE false skips the substitution: gbar is v itself (the smoother's VJP solves the stacked system of the whole clip and
+// runs only the target pass here, after H_q, the targets and the links of the frame are in the scratch; kA is not read).
+template <int G, bool SOLVE = true>
 __device__ __forceinline__ VjpLane vjp_tail(Solver<G, 0>& sv, const FrameInputs& in_, const Dims& dm, const VjpFront& fr,
                                             float gbar, float* grad_ref, bool active) {
   using VS = VjpScratch<G>;
@@ -2024,15 +2026,17 @@ __device__ __forceinline__ VjpLane vjp_tail(Solver<G, 0>& sv, const FrameInputs&
 
   // v = A^-1 gbar (forward, then back substitution; frozen rows are identity rows with a zero right-hand side)
   float y = free_ ? gbar : 0.f;
-  for (int k = 0; k < dof; ++k) {
-    const float yk = gshfl<G>(y, k) / A[k * (NP + 1) + k];
-    if (l == k) y = yk;
-    else if (l > k && l < dof) y = fmaf(-A[l * (NP + 1) + k], yk, y);
-  }
-  for (int k = dof - 1; k >= 0; --k) {
-    const float vk = gshfl<G>(y, k) / A[k * (NP + 1) + k];
-    if (l == k) y = vk;
-    else if (l < k) y = fmaf(-A[k * (NP + 1) + l], vk, y);
+  if constexpr (SOLVE) {
+    for (int k = 0; k < dof; ++k) {
+      const float yk = gshfl<G>(y, k) / A[k * (NP + 1) + k];
+      if (l == k) y = yk;
+      else if (l > k && l < dof) y = fmaf(-A[l * (NP + 1) + k], yk, y);
+    }
+    for (int k = dof - 1; k >= 0; --k) {
+      const float vk = gshfl<G>(y, k) / A[k * (NP + 1) + k];
+      if (l == k) y = vk;
+      else if (l < k) y = fmaf(-A[k * (NP + 1) + l], vk, y);
+    }
   }
   const float v = bad ? 0.f : y;
   {
@@ -2855,6 +2859,221 @@ __device__ __forceinline__ void smooth_packed_stream(Solver<G, 0>& sv, const dex
     }
   }
   if (has && io.cost_out && l == 0) io.cost_out[sc] = nonfinite ? __int_as_float(0x7fc00000) : F;
+  __syncwarp();
+}
+
+// ------------------------------------------------------------------------------------------------
+// backpropagation through the offline smoother (dexr_smooth_sequences_packed_vjp): one linear solve per stream
+// ------------------------------------------------------------------------------------------------
+// The argument checks of dexr_smooth_sequences_packed_vjp: nullptr, or what is wrong.  Host code shared by the library and
+// the host emulation.  offsets live on the device and are not read here.
+inline const char* smooth_vjp_io_error(const dexr_table_t& t, const dexr_smooth_vjp_t& io, const dexr_params_t& prm,
+                                       const int64_t* offsets, long long S, long long N) {
+  if (S < 0 || N < 0 || N > INT32_MAX) return "bad sizes: num_streams and num_frames must be >= 0, num_frames <= INT32_MAX";
+  if (!offsets) return "offsets (device [S+1]) are required";
+  if (prm.preprocess != 0) return "raw landmarks are not differentiated: params.preprocess must be 0 (pre-process the keypoints first)";
+  if (!io.keypoints || !io.qpos || !io.grad_keypoints) return "keypoints, qpos and grad_keypoints are required";
+  if (t.n_fixed > 0 && !io.fixed_qpos) return "the robot has fixed joints but fixed_qpos is NULL";
+  if (io.grad_last_qpos && !io.last_qpos) return "grad_last_qpos needs last_qpos";
+  if (!(io.smooth_weight < 0.f) && !(io.smooth_weight >= 0.f && io.smooth_weight <= 3.0e38f))
+    return "smooth_weight must be finite (< 0: params.norm_delta)";
+  if (N > 0 && (!io.workspace || io.workspace_bytes < smooth_workspace_bytes(t, N)))
+    return "workspace smaller than dexr_smooth_workspace_bytes(robot, num_frames)";
+  return nullptr;
+}
+
+// Packed stream `si` of `pk` (none when out of range) of dexr_smooth_sequences_packed_vjp (see dexr.h for the math); `owner`
+// as in smooth_packed_stream.  Three sweeps along the clip, every frame at the given point X*:
+//   forward   targets (the DexPilot flag recurrence), FK, H_q and the data gradient (smooth_eval, exact_grad_hq: the
+//             smoother's own forward sweep with mu = 0, the exact model only), the active set on the total gradient, then
+//             block Thomas: S_t = D_t - (2w)^2 Z_{t-1}, y_t = G_t + 2w Z_{t-1} y_{t-1}; Z_t and y_t into the workspace;
+//   backward  v_t = Z_t (y_t + 2w v_{t+1}) into the workspace (the smoother's kX slot);
+//   cotangent the frame again (targets, FK, H_q), then vjp_tail's target pass and fixed-joint term with v_t.
+// The stream's NONFINITE and NOT_PD verdicts are known after the forward sweep and select every output.  `dm` and `ws` as in
+// smooth_packed_stream; sv.prm.norm_delta holds w.
+template <int G>
+__device__ __forceinline__ void smooth_vjp_packed_stream(Solver<G, 0>& sv, const dexr_smooth_vjp_t& io, const Dims& dm,
+                                                         const PackedLayout& pk, long long si, bool owner) {
+  using W = SmoothWs<G>;
+  constexpr int NP = G;
+  const SharedTable& st = Solver<G, 0>::ST();
+  const int l = sv.l, lane = sv.lane, dof = dm.dof, n = dm.n_var;
+  const bool isvar = sv.var >= 0, isjoint = l < dof;
+  const PackedStream ps = packed_stream(pk, si);
+  const bool valid = owner && ps.s >= 0;
+  const int len = valid ? ps.len : 0;
+  const int steps = warp_steps<G>(len);
+  const bool has = len > 0;
+  const long long sc = si;  // (read only where `valid` holds: the caller's loop index, no register of its own)
+  const int f0 = has ? (int)ps.first : 0;  // (num_frames <= INT32_MAX: 32 bits, one register fewer)
+  const int tlast = has ? len - 1 : 0;
+  // (the workspace is addressed from io.workspace per frame: a kernel argument, so no register holds its base)
+  float* const A = sv.scf() + VjpScratch<G>::kA;
+  float* const hq = sv.scf() + VjpScratch<G>::kH;
+  const float w = sv.prm.norm_delta, w2 = 2.0f * w;
+  const bool anchor = io.last_qpos != nullptr;
+  // the forward's view of the inputs, for the smoother's frame helpers
+  dexr_smooth_t fio{};
+  fio.keypoints = io.keypoints;
+  fio.fixed_qpos = io.fixed_qpos;
+  fio.projected = io.projected;
+
+  // G_t of this lane's variable at frame fr (0 off the variables), and `gq`, this lane's joint's grad_robot_qpos
+  auto cotangent = [&](long long fr, bool live, float& gq) -> float {
+    gq = (live && isjoint && io.grad_robot_qpos) ? io.grad_robot_qpos[fr * dof + l] : 0.f;
+    float gb = gq;
+    if (dm.has_mimic) {
+      const int gcount = st.group_count[l];
+      float gx_ = 0.f;
+#pragma unroll
+      for (int k = 0; k < DEXR_MAX_GROUP; ++k) {
+        const bool v = isvar && k < gcount;
+        const float gv = gshfl<G>(gq, v ? st.group_lane[l][k] : l);
+        if (v) gx_ = fmaf(st.group_mult[l][k], gv, gx_);
+      }
+      gb = gx_;
+    }
+    if (live && isvar && io.grad_qpos) gb += io.grad_qpos[fr * n + sv.var];
+    return isvar ? gb : 0.f;
+  };
+
+  // ---- the clipped anchor
+  auto raw_anchor = [&]() { return (has && isvar && anchor) ? io.last_qpos[sc * n + sv.var] : 0.f; };
+  auto clipped_anchor = [&]() { return fminf(fmaxf(raw_anchor(), st.clip_lo[l]), st.clip_hi[l]); };
+  bool nonfinite = !isfinite(raw_anchor());
+
+  // ---- forward sweep: the elimination of H V = G.  G_t waits in the workspace's kG slot while the frame is evaluated, and
+  // only the smoothness gradient of the neighbours stays in registers (the 16-lane kernel has 128 of them)
+  smooth_reset_flags(sv, fio, dm, sc, has);
+  bool bad = false;
+  float yprev = 0.f;
+  for (int t = 0; t < steps; ++t) {
+    const bool live = t < len;
+    const int tc = t < tlast ? t : tlast;
+    const long long fr = (long long)(f0 + tc);
+    float* const wt = static_cast<float*>(io.workspace) + (long long)(f0 + tc) * W::kFloats;
+    const bool missing = smooth_missing(sv, fio, dm, fr, live);
+    const bool has_prev = t > 0 || anchor, has_next = t + 1 < len;
+    {
+      float gq;
+      const float gb = cotangent(fr, live, gq);
+      nonfinite = nonfinite || !isfinite(gb) || !isfinite(gq);
+      if (live) wt[W::kG + l] = gb;
+    }
+    float x = 0.f, xp = t > 0 ? 0.f : clipped_anchor(), xn = 0.f;
+    if (live && isvar) {
+      x = io.qpos[fr * n + sv.var];
+      if (t > 0) xp = io.qpos[(fr - 1) * n + sv.var];
+      if (has_next) xn = io.qpos[(fr + 1) * n + sv.var];
+    }
+    nonfinite = nonfinite || !isfinite(x);
+    const float gs = (has_prev ? w2 * (x - xp) : 0.f) + (has_next ? w2 * (x - xn) : 0.f);
+    smooth_eval(sv, fio, dm, fr, x, xp, has_prev, missing, live);
+    float g = exact_grad_hq(sv, dm);
+    if (missing) {
+      g = 0.f;
+#pragma unroll
+      for (int i = 0; i < NP; ++i) hq[i * NP + l] = 0.f;
+    }
+    g = isvar ? g + gs : 0.f;
+    const bool at_bound = isvar && ((x <= sv.lo && g > -kGradNoise) || (x >= sv.hi && g < kGradNoise));
+    const bool free_ = live && isvar && !at_bound;
+    const unsigned fmask = gballot<G>(free_, lane);
+    __syncwarp();
+    fold_free_block(sv, dm, A, free_, fmask, w2 * (float)((has_prev ? 1 : 0) + (has_next ? 1 : 0)));
+    float y = (free_ && live) ? wt[W::kG + l] : 0.f;
+    if (t > 0) {  // (warp-uniform) the Schur complement of frame t - 1: Z_{t-1} is zero off its free variables
+      const float* zp = wt - W::kFloats + W::kZ;
+      float zy = 0.f;
+      for (int c = 0; c < dof; ++c) {
+        const float z = live ? zp[c * G + l] : 0.f;
+        zy = fmaf(z, gshfl<G>(yprev, c), zy);
+        if (free_ && ((fmask >> c) & 1u)) A[l * (NP + 1) + c] = fmaf(-w2 * w2, z, A[l * (NP + 1) + c]);
+      }
+      if (free_) y = fmaf(w2, zy, y);
+    }
+    const bool pb = factor_rows<G>(A, dof, l);
+    __syncwarp();
+    bad = bad || (live && pb);
+    // Z_t, column l, as in smooth_packed_stream (z in the kH area, H_q is folded into A by now)
+    for (int k = 0; k < dof; ++k) {
+      float s = k == l ? 1.0f : 0.f;
+      for (int i = 0; i < k; ++i) s = fmaf(-A[k * (NP + 1) + i], hq[i * NP + l], s);
+      hq[k * NP + l] = s / A[k * (NP + 1) + k];
+    }
+    for (int k = dof - 1; k >= 0; --k) {
+      float s = hq[k * NP + l];
+      for (int i = k + 1; i < dof; ++i) s = fmaf(-A[i * (NP + 1) + k], hq[i * NP + l], s);
+      s = s / A[k * (NP + 1) + k];
+      hq[k * NP + l] = s;
+      if (live) wt[W::kZ + k * G + l] = (free_ && ((fmask >> k) & 1u)) ? s : 0.f;
+    }
+    if (live) wt[W::kY + l] = y;
+    yprev = y;
+    __syncwarp();  // the next frame rewrites the scratch this one read
+  }
+  nonfinite = gany<G>(nonfinite, lane);
+
+  // ---- backward sweep: v_t
+  float vn = 0.f;
+  for (int t = steps - 1; t >= 0; --t) {
+    const bool live = t < len;
+    const int tc = t < tlast ? t : tlast;
+    float* const wt = static_cast<float*>(io.workspace) + (long long)(f0 + tc) * W::kFloats;
+    const float r = live ? wt[W::kY + l] + (t + 1 < len ? w2 * vn : 0.f) : 0.f;
+    float d = 0.f;
+    for (int c = 0; c < dof; ++c) d = fmaf(live ? wt[W::kZ + c * G + l] : 0.f, gshfl<G>(r, c), d);
+    if (live) {
+      wt[W::kX + l] = d;
+      vn = d;
+    }
+  }
+
+  // ---- cotangent sweep: the target pass and the fixed-joint term of every frame with its v_t
+  smooth_reset_flags(sv, fio, dm, sc, has);
+  for (int t = 0; t < steps; ++t) {
+    const bool live = t < len;
+    const int tc = t < tlast ? t : tlast;
+    const long long fr = (long long)(f0 + tc);
+    const float* const wt = static_cast<float*>(io.workspace) + (long long)(f0 + tc) * W::kFloats;
+    const bool missing = smooth_missing(sv, fio, dm, fr, live);
+    float x = 0.f, xp = t > 0 ? 0.f : clipped_anchor();
+    if (live && isvar) {
+      x = io.qpos[fr * n + sv.var];
+      if (t > 0) xp = io.qpos[(fr - 1) * n + sv.var];
+    }
+    smooth_eval(sv, fio, dm, fr, x, xp, t > 0 || anchor, missing, live);
+    if (dm.n_fixed > 0) exact_grad_hq(sv, dm);  // (H_q into kH, for the fixed-joint term only; the gradient is not needed)
+    FrameInputs in;
+    in.kp = io.keypoints + fr * (3 * DEXR_NUM_KEYPOINTS);
+    in.ref = nullptr;
+    in.fixed = nullptr;
+    in.last = nullptr;
+    in.projected = nullptr;
+    const float v = (live && isvar) ? wt[W::kX + l] : 0.f;
+    const VjpLane r = vjp_tail<G, false>(sv, in, dm, VjpFront{isvar, true, false}, v, nullptr, live);
+    // outputs: NaN for a non-finite stream, 0 for a NOT_PD one and on a missing frame
+    auto out = [&](float val) { return nonfinite ? __int_as_float(0x7fc00000) : ((bad || missing) ? 0.f : val); };
+    if (live) {
+      const int fixedi = st.fixed_index[l];
+      const float* const kpacc = sv.scf() + VjpScratch<G>::kKp;
+      const int base_status = nonfinite ? DEXR_STATUS_NONFINITE : (bad ? DEXR_STATUS_NOT_PD : 0);
+      const float gqd = (fixedi >= 0 && io.grad_robot_qpos) ? io.grad_robot_qpos[fr * dof + l] : 0.f;
+      if (fixedi >= 0 && io.grad_fixed_qpos) io.grad_fixed_qpos[fr * dm.n_fixed + fixedi] = out(gqd - r.qbar);
+      for (int e = l; e < 3 * DEXR_NUM_KEYPOINTS; e += G) io.grad_keypoints[fr * 3 * DEXR_NUM_KEYPOINTS + e] = out(kpacc[e]);
+      if (l == 0 && io.status_out) io.status_out[fr] = base_status | (missing ? DEXR_STATUS_MISSING : 0);
+    }
+    __syncwarp();  // the next frame rewrites the scratch this one read
+  }
+  // ---- the anchor: 2 w v_0 where the clip passes it (an empty or malformed range: 0); v_0 is read back from the workspace
+  // rather than held in a register through the cotangent sweep
+  if (valid && isvar && io.grad_last_qpos) {
+    const float ar = raw_anchor();
+    const bool passes = ar >= st.clip_lo[l] && ar <= st.clip_hi[l];
+    const float v0 = has ? static_cast<const float*>(io.workspace)[(long long)f0 * W::kFloats + W::kX + l] : 0.f;
+    const float ga = nonfinite ? __int_as_float(0x7fc00000) : ((bad || !passes) ? 0.f : w2 * v0);
+    io.grad_last_qpos[sc * n + sv.var] = has ? ga : 0.f;
+  }
   __syncwarp();
 }
 

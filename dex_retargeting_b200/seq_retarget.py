@@ -645,3 +645,68 @@ class SeqRetargeting:
                                                      C.c_void_p(s.cuda_stream)), "dexr_smooth_sequences_packed")
         ws.record_stream(s)
         return out, qpos, status_out
+
+    def smooth_packed_sequences_vjp(self, keypoints, layout: PackedStreams, qpos, last_qpos0=None, projected0=None,
+                                    grad_qpos=None, grad_robot_qpos=None, *, fixed_qpos=None, smooth_weight=None,
+                                    grad_keypoints_out=None, grad_fixed_qpos_out=None, grad_last_qpos_out=None,
+                                    status_out=None, stream=None):
+        """Backpropagation through `smooth_packed_sequences` (`dexr_smooth_sequences_packed_vjp`, one launch): the
+        implicit-function VJP of the smoothed clips `qpos` [N,opt_dof] (the forward's answer) with respect to the keypoints,
+        the fixed joints and the anchor.  Per-frame tensors [N,...] (keypoints, fixed_qpos, qpos, grad_qpos,
+        grad_robot_qpos, status_out and the returned grad_keypoints / grad_fixed_qpos), per-stream ones [S,...]
+        (last_qpos0 and projected0: the forward's `state.last_qpos` and `state.projected`; the returned grad_last_qpos).
+        `smooth_weight` as given to the forward.  Returns (grad_keypoints [N,21,3], grad_fixed_qpos [N,n_fixed] or None,
+        grad_last_qpos [S,opt_dof] or None when last_qpos0 is None).  The gradient is not causal: a loss on one frame
+        reaches the keypoints of every frame of its stream.  A stream whose stacked Hessian is not positive definite gets
+        zero gradients (STATUS_NOT_PD), one with a non-finite qpos, anchor or cotangent NaN (STATUS_NONFINITE).
+        Allocates its workspace on the device; nothing is synchronised."""
+        import torch
+
+        opt = self.optimizer
+        eng = opt.engine()
+        dev = torch.device("cuda", eng.device)
+        S, N_ = layout.num_streams, layout.num_frames
+        n, dof, nf = opt.opt_dof, opt.robot.dof, len(opt.idx_pin2fixed)
+        chk = _checker(dev)
+
+        def out(t, shape, name):
+            t = torch.empty(shape, dtype=torch.float32, device=dev) if t is None else t
+            return t, chk(t, shape, torch.float32, name)
+
+        io = N.DexrSmoothVjp()
+        io.keypoints = chk(keypoints, (N_, N.NUM_KEYPOINTS, 3), torch.float32, "keypoints")
+        if nf:
+            if fixed_qpos is None:
+                raise ValueError(f"Optimizer has {nf} fixed joints but no fixed_qpos is given")
+            io.fixed_qpos = chk(fixed_qpos, (N_, nf), torch.float32, "fixed_qpos")
+        if last_qpos0 is not None:
+            io.last_qpos = chk(last_qpos0, (S, n), torch.float32, "last_qpos0")
+        if projected0 is not None:
+            io.projected = chk(projected0, (S, projected0.shape[1]), torch.uint8, "projected0")
+        io.qpos = chk(qpos, (N_, n), torch.float32, "qpos")
+        if grad_qpos is not None:
+            io.grad_qpos = chk(grad_qpos, (N_, n), torch.float32, "grad_qpos")
+        if grad_robot_qpos is not None:
+            io.grad_robot_qpos = chk(grad_robot_qpos, (N_, dof), torch.float32, "grad_robot_qpos")
+        io.smooth_weight = -1.0 if smooth_weight is None else float(smooth_weight)
+        g_kp, io.grad_keypoints = out(grad_keypoints_out, (N_, N.NUM_KEYPOINTS, 3), "grad_keypoints_out")
+        g_fixed = None
+        if nf:
+            g_fixed, io.grad_fixed_qpos = out(grad_fixed_qpos_out, (N_, nf), "grad_fixed_qpos_out")
+        g_last = None
+        if last_qpos0 is not None:
+            g_last, io.grad_last_qpos = out(grad_last_qpos_out, (S, n), "grad_last_qpos_out")
+            if N_ == 0:  # (the library does nothing for 0 frames: every stream is empty)
+                g_last.zero_()
+        if status_out is not None:
+            io.status_out = chk(status_out, (N_,), torch.int32, "status_out")
+        offsets = chk(layout.offsets, (S + 1,), torch.int64, "layout.offsets")
+        nbytes = int(eng.lib.dexr_smooth_workspace_bytes(eng.handle, N_))
+        ws = torch.empty((max(nbytes, 4),), dtype=torch.uint8, device=dev)
+        io.workspace, io.workspace_bytes = ws.data_ptr(), nbytes
+        s = stream if stream is not None else torch.cuda.current_stream(dev)
+        p = opt.params(clip_init=True, lp_alpha=self.low_pass_alpha)
+        N.check(eng.lib.dexr_smooth_sequences_packed_vjp(eng.handle, C.byref(p), C.byref(io), C.c_void_p(offsets), S, N_,
+                                                         C.c_void_p(s.cuda_stream)), "dexr_smooth_sequences_packed_vjp")
+        ws.record_stream(s)
+        return g_kp, g_fixed, g_last

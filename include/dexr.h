@@ -465,6 +465,62 @@ int dexr_smooth_sequences_packed(const dexr_robot_t* robot, const dexr_params_t*
                                  const int64_t* offsets /* device [S+1] */, int64_t num_streams, int64_t num_frames,
                                  void* cuda_stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Backpropagation through the offline smoother: the implicit-function VJP of dexr_smooth_sequences_packed's answer with
+ * respect to the keypoints, the fixed joints and the anchor, every packed stream in one launch.  Per stream, X* = (x_0 ..
+ * x_{T-1}) (`qpos`, the smoother's answer) is taken as a stationary point, on its free variables, of the smoother's
+ *   F(X; theta) = sum_t L_t(x_t; kp_t, fixed_t) + w sum_{t>=1} |x_t - x_{t-1}|^2 + w |x_0 - clip(a)|^2,
+ * theta = (keypoints, fixed joints, anchor a), w = smooth_weight (< 0: params.norm_delta).  Given G = dl/dX:
+ *   1. G_t = grad_qpos_t + M^T grad_robot_qpos_t (mimic followers folded into their source; a fixed joint's share of
+ *      grad_robot_qpos goes straight to grad_fixed_qpos);
+ *   2. the active set is the smoother's rule on the TOTAL gradient (data + smoothness + anchor) at X*, at the widened bounds:
+ *      active variables get zero sensitivity;
+ *   3. H V = G over the free variables, H the exact block-tridiagonal Hessian of F (diagonal blocks D_t = M^T H_q M +
+ *      2 w k_t I, k_t the frame's neighbours with the anchor counting as one; off-diagonal blocks -2 w I; no damping, no
+ *      Gauss-Newton fallback), by block Thomas along the clip: S_t = D_t - (2w)^2 Z_{t-1}, y_t = G_t + 2w Z_{t-1} y_{t-1},
+ *      then v_t = Z_t (y_t + 2w v_{t+1}), Z_t the inverse of S_t over the free variables of frame t;
+ *   4. theta_bar = -(dg/dtheta)^T V, frame by frame: grad_keypoints_t is dexr_solve_vjp's target pass run with v_t,
+ *      grad_fixed_qpos_t = -H_q[c, :] . M v_t plus the direct term of step 1, and the anchor's
+ *      grad_last_qpos = 2 w v_0 where clip_lo <= a <= clip_hi (inclusive, as torch.clamp), 0 elsewhere.
+ * Not differentiated: the DexPilot flags (the forward's hysteresis recurrence along the clip from projected[s], read only),
+ * the starting trajectory (it only picks the basin) and w.  The gradient is NOT causal: a loss on frame t reaches the
+ * keypoints of every frame of its stream.
+ *   NOT_PD: at a strict local minimum the stacked free Hessian is positive definite, and so is every Schur complement; a
+ *     pivot <= 0 anywhere in the elimination means X* is not one.  That stream gets zero cotangents and DEXR_STATUS_NOT_PD
+ *     on every frame.  A stream the forward left at DEXR_STATUS_MAXITER gets the derivative of the linearisation at the
+ *     point given.
+ *   NONFINITE: the solve couples all frames of a stream, so a non-finite qpos, anchor or cotangent makes the whole stream's
+ *     cotangents NaN (grad_last_qpos included) with DEXR_STATUS_NONFINITE; other streams are not affected.
+ *   Missing frames (a non-finite keypoint or fixed joint: DEXR_STATUS_MISSING, as in the forward) have no data term but
+ *     still carry the chain through their smoothness terms; their keypoint and fixed-joint cotangents are 0, not NaN.
+ *   status_out: 0, DEXR_STATUS_NOT_PD or DEXR_STATUS_NONFINITE, | DEXR_STATUS_MISSING on a missing frame.
+ *   Layout: the packed rules of dexr_smooth_sequences_packed; an empty or malformed range writes nothing in the per-frame
+ *     arrays, and its grad_last_qpos row is 0.  Raw landmarks (params.preprocess != 0) are refused.
+ *   `workspace`: the forward's, at least dexr_smooth_workspace_bytes(robot, num_frames) bytes (DEXR_E_INVALID below): Z_t,
+ *     y_t and v_t fit in its per-frame block.  The call is asynchronous on `cuda_stream` and allocates nothing.  All
+ *     pointers are DEVICE pointers.
+ * ------------------------------------------------------------------------------------------- */
+typedef struct dexr_smooth_vjp {
+  const float* keypoints;       /* [N,21,3] as given to the forward                                                     */
+  const float* fixed_qpos;      /* [N,n_fixed] or NULL when n_fixed == 0                                                */
+  const float* last_qpos;       /* [S,n_var] the anchor a as given to the forward, or NULL: no anchor term              */
+  const uint8_t* projected;     /* [S,len_proj] DexPilot flags at the start of each stream, as given to the forward     */
+  const float* qpos;            /* [N,n_var] the smoother's answer X*                                                   */
+  const float* grad_qpos;       /* [N,n_var] dl/dqpos, or NULL (= 0)                                                    */
+  const float* grad_robot_qpos; /* [N,dof] dl/drobot_qpos, or NULL (= 0)                                                */
+  float smooth_weight;          /* w as given to the forward; < 0: params.norm_delta                                    */
+  void* workspace;              /* device scratch of at least dexr_smooth_workspace_bytes(robot, num_frames) bytes      */
+  size_t workspace_bytes;
+  float* grad_keypoints;        /* [N,21,3] (all 63 entries of every frame of a non-empty stream written)               */
+  float* grad_fixed_qpos;       /* [N,n_fixed] or NULL                                                                  */
+  float* grad_last_qpos;        /* [S,n_var] or NULL (needs last_qpos)                                                  */
+  int32_t* status_out;          /* [N] or NULL                                                                          */
+} dexr_smooth_vjp_t;
+size_t dexr_smooth_vjp_sizeof(void);
+int dexr_smooth_sequences_packed_vjp(const dexr_robot_t* robot, const dexr_params_t* params, const dexr_smooth_vjp_t* io,
+                                     const int64_t* offsets /* device [S+1] */, int64_t num_streams, int64_t num_frames,
+                                     void* cuda_stream);
+
 #ifdef __cplusplus
 }
 #endif
