@@ -348,20 +348,22 @@ __device__ inline void load_shared_table(SharedTable& st, const dexr_table_t* __
 // ------------------------------------------------------------------------------------------------
 // per-group scratch in shared memory (floats)
 // ------------------------------------------------------------------------------------------------
-// BW: the Solver<G, BW> instantiation the group runs.  Block mode (BW > 0) backs up and transposes only the BW-column row
-// segments its lanes hold (2.3 KB instead of 3.9 KB per 16-lane group: room for more consumer warps next to the ring);
+// BW: the Solver<G, BW> instantiation the group runs.  Block mode (BW > 0) backs up only the BW-column row segments its
+// lanes hold and factorises every block in registers, so it needs no transposed factor: its last area holds the NP
+// right-hand sides instead (2.1 KB instead of 3.9 KB per 16-lane group: room for more consumer warps next to the ring);
 // dense mode needs all NP rows (and the mimic-fold temporaries), arrow mode keeps its Schur matrix in the backup area.
 template <int G, int BW = 0>
 struct Scratch {
   static constexpr int NP = G;
-  static constexpr int kRows = BW > 0 ? BW : NP;                // rows of the backup and of the transposed factor
+  static constexpr int kRows = BW > 0 ? BW : NP;                // rows of the backup
   static constexpr int kFr = 0;                                 // [MAX_RES][4] target xyz, weight c_k
   static constexpr int kLp = kFr + DEXR_MAX_RES * 4;            // [2][MAX_LINKS][4] link positions
   static constexpr int kU = kLp + 2 * DEXR_MAX_LINKS * 4;       // jbuf[2][3][NP] (aliased by the 2 Cholesky row buffers) + at: 2 x [NP + NP/4] float4
   static constexpr int kUSize = 16 * NP;
   static constexpr int kHb = kU + kUSize;                       // [kRows][NP]   Hessian backup, column per lane
-  static constexpr int kLcol = kHb + kRows * NP;                // [kRows][NP+1] L^T rows, conflict-free column reads (also mimic-fold temp)
-  static constexpr int kFloats = ((kLcol + kRows * (NP + 1) + 3) / 4) * 4;
+  static constexpr int kLcol = kHb + kRows * NP;                // [NP][NP+1] L^T rows, conflict-free column reads (also mimic-fold temp)
+  static constexpr int kRhs = kLcol;                            // block mode: [NP] -g of every lane, the blocks' right-hand sides
+  static constexpr int kFloats = ((kLcol + (BW > 0 ? NP : kRows * (NP + 1)) + 3) / 4) * 4;
   static constexpr int kStreamFloats = kFloats + 64;  // sequences: followed by the current frame's 63 keypoint floats
 };
 
@@ -380,11 +382,13 @@ struct FrameInputs {
 // frames kernel runs at 80 registers): two words instead of eleven registers carried through every phase of an iteration.
 //   w0: bits 0-15 iterations, 16-22 rejected trials (saturated at 127), 23-25 the status flags, 26 done, 27 exact,
 //       28 recheck, 29 trust_prev, 30-31 stall (saturated at 3: only `stall >= 2` is read)
-//   w1: bits 0-15 the free-variable mask of the previous iteration, 16-17 rechecks (at most 3)
+//   w1: bits 0-15 the free-variable mask of the previous iteration, 16-30 rechecks (at most 3), 31 the step accepted in this
+//       iteration was below kNearStep (kNear: inc_rechecks() masks it out of the count)
 // w0 & 0x3ffffff is the status word (dexr.h).  Unpacked: one variable each.
 template <bool P>
 struct Bookkeeping {
   static constexpr uint32_t kDone = 1u << 26, kExact = 1u << 27, kRecheck = 1u << 28, kTrust = 1u << 29;
+  static constexpr uint32_t kNear = 1u << 31;  // (w1)
   uint32_t w0 = kExact, w1 = 0;
   int iters_ = 0, rejects_ = 0, rechecks_ = 0, stall_ = 0, status_ = 0;
   unsigned last_fmask_ = 0u;
@@ -430,8 +434,11 @@ struct Bookkeeping {
     if constexpr (P) w1 = (w1 & ~0xffffu) | m;
     else last_fmask_ = m;
   }
+  // packed only (the unpacked solver keeps the accepted step itself)
+  __device__ __forceinline__ bool near() const { return (w1 & kNear) != 0u; }
+  __device__ __forceinline__ void set_near(bool x) { w1 = x ? (w1 | kNear) : (w1 & ~kNear); }
   __device__ __forceinline__ int inc_rechecks() {  // ++rechecks
-    if constexpr (P) { w1 += 1u << 16; return (int)(w1 >> 16); }
+    if constexpr (P) { w1 += 1u << 16; return (int)((w1 >> 16) & 0x7fffu); }
     else return ++rechecks_;
   }
   // the status word: flags, iterations and rejected trials (saturated at 127)
@@ -538,6 +545,7 @@ struct Solver {
   __device__ __forceinline__ float4& at_t(int i) const { return reinterpret_cast<float4*>(scf() + SC::kU + 6 * NP)[NP + NP / 4 + at_slot(i)]; }
   __device__ __forceinline__ float* lrow() const { return scf() + SC::kU; }
   __device__ __forceinline__ float* hb() const { return scf() + SC::kHb; }
+  // the transposed factor (dense, arrow) or the mimic-fold temporary (dense); block mode has no such area: there kLcol is kRhs
   __device__ __forceinline__ float* lcol() const { return scf() + SC::kLcol; }
 
   // q of every joint from the variables: target joints copy, fixed joints constant, mimic affine.
@@ -1087,6 +1095,7 @@ struct Solver {
       float* hbuf = hb();
 #pragma unroll
       for (int i = 0; i < HN; ++i) hbuf[i * NP + l] = H[i];
+      if constexpr (BW > 0) scf()[SC::kRhs + l] = -g;  // every lane of a window solves the window's whole block
       // own diagonal entry (register index = lane id is not addressable: read it back from the column store);
       // the regulariser 2*norm_delta enters on the diagonal at pivot time together with the damping
       const float reg2 = free_ ? 2.0f * nd : 0.f;
@@ -1100,18 +1109,69 @@ struct Solver {
       for (int trial = 0; trial < kMaxTrials; ++trial) {
         if (!gany<32>(!accepted, lane)) break;
         refresh();
-        // block mode reads H back from the backup on the first trial too (the same values) instead of holding it in registers
-        // through the active-set and trust bookkeeping
-        if (trial > 0 || BW > 0) {
+        // (block mode factorises straight from the backup and does not hold H in registers through the trials at all)
+        if (BW <= 0 && trial > 0) {
 #pragma unroll
           for (int i = 0; i < HN; ++i) H[i] = hbuf[i * NP + l];
         }
         float y = -g;
         float myinv = 1.0f;
         bool bad = false;
-        float* Lr = lrow();   // two NP-float row buffers, alternating per pivot
+        // dense and arrow modes only: two NP-float row buffers, alternating per pivot, and the transposed factor.  Block mode
+        // uses neither -- its kLcol area is kRhs, the right-hand sides the block factorisation reads -- and must not write
+        // through them.
+        float* Lr = lrow();
         float* Lc = lcol();
-        __syncwarp();
+        __syncwarp();  // (block mode: the backup and right-hand-side stores of the other rows of the window)
+        if constexpr (BW > 0) {
+          // ================= block factorisation: every window's 4 x 4 block in registers =================
+          // Every lane of a window factorises and solves the window's block redundantly (Cholesky, forward and back
+          // substitution) from the backup, which holds entry (r, c) of the block as row r stored it -- H is not bitwise
+          // symmetric, so only the lower triangle, r >= c, is read, as the dense pivot loop below reads it.  The operations
+          // and their order are the pivot loop's for bw = 4, so the step is the same to the bit; what goes away is its
+          // per-pivot traffic: two shuffles, two row-buffer stores, a warp barrier and a row load per pivot, and four
+          // shuffles and loads in the back substitution.
+          static_assert(BW == 4, "the register factorisation is written for 4-joint windows");
+          // Written column by column (left looking), the substitutions after the factorisation: every entry sees the same
+          // updates in the same order (pivot 0, 1, ...) as in the pivot loop.
+          // (the window's first lane is formed from the lane index refresh() just unpacked, not from the iteration's cb: what
+          // derives from it -- the rows' free bits and regularisers -- is then formed here rather than held through the trials)
+          const int wb = l & ~(BW - 1);
+          const float* hw = hb() + wb;  // hw[j * NP + r]: entry (r, j) of this window's block
+          // the damping + regulariser row r adds to its pivot, d_r = a_rr + fmaf(lam, D, reg2) with hd, D and reg2 as lane wb + r
+          // forms them from its stored diagonal entry hrr
+          auto pivot = [&](int r, float hrr, float arr) {
+            const bool fr = (fmask >> (wb + r)) & 1u;
+            const float rg = fr ? 2.0f * nd : 0.f;
+            const float d = arr + fmaf(lam, fabsf(fr ? hrr + rg : 1.0f) + 1e-6f, rg);
+            bad = bad || !(d > 1e-20f);
+            return fast_rsqrt(fmaxf(d, 1e-20f));
+          };
+          const float4 c0 = *reinterpret_cast<const float4*>(hw);
+          const float i0 = pivot(0, c0.x, c0.x);
+          const float l10 = c0.y * i0, l20 = c0.z * i0, l30 = c0.w * i0;
+          const float4 c1 = *reinterpret_cast<const float4*>(hw + NP);
+          const float i1 = pivot(1, c1.y, fmaf(-l10, l10, c1.y));
+          const float l21 = fmaf(-l20, l10, c1.z) * i1, l31 = fmaf(-l30, l10, c1.w) * i1;
+          const float4 c2 = *reinterpret_cast<const float4*>(hw + 2 * NP);
+          const float i2 = pivot(2, c2.z, fmaf(-l21, l21, fmaf(-l20, l20, c2.z)));
+          const float l32 = fmaf(-l31, l21, fmaf(-l30, l20, c2.w)) * i2;
+          const float h33 = hw[3 * NP + 3];
+          const float i3 = pivot(3, h33, fmaf(-l32, l32, fmaf(-l31, l31, fmaf(-l30, l30, h33))));
+          // forward substitution, L z = -g
+          const float4 rhs = *reinterpret_cast<const float4*>(scf() + SC::kRhs + wb);
+          const float z0 = rhs.x * i0;
+          const float z1 = fmaf(-l10, z0, rhs.y) * i1;
+          const float z2 = fmaf(-l21, z1, fmaf(-l20, z0, rhs.z)) * i2;
+          const float z3 = fmaf(-l32, z2, fmaf(-l31, z1, fmaf(-l30, z0, rhs.w))) * i3;
+          // back substitution, L^T delta = z
+          const float x3 = z3 * i3;
+          const float x2 = fmaf(-l32, x3, z2) * i2;
+          const float x1 = fmaf(-l21, x2, fmaf(-l31, x3, z1)) * i1;
+          const float x0 = fmaf(-l10, x1, fmaf(-l20, x2, fmaf(-l30, x3, z0))) * i0;
+          const int r = l - wb;
+          y = r == 0 ? x0 : (r == 1 ? x1 : (r == 2 ? x2 : x3));
+        }
         // Cholesky, lane = row, as a ROLLED loop: after pivot k every lane shifts its row one column to the
         // left (fused into the update FMA), so the pivot column is always register H[0] and the loop body is
         // the same code for every k -- 16-32x less code than the unrolled form (instruction-cache bound
@@ -1246,12 +1306,12 @@ struct Solver {
             }
           }
         }
-        if constexpr (!AR) {
+        if constexpr (dense) {
           // One pivot step, with the number of 4-column chunks of the rotating window it updates fixed at compile time.  The
           // window shrinks by one column per pivot, so the steps are run in PHASES of decreasing chunk count (HN = 16: 4, 3,
           // 2, 1 chunks while more than 12, 8, 4, 0 columns are live) instead of predicating all HN / 4 chunks off one by
           // one: half of the FFMA / LDS.128 issue slots of a 16 x 16 factorisation went into predicated-off instructions.
-          constexpr int kMask = dense ? NP - 1 : BW - 1;
+          constexpr int kMask = NP - 1;
           const float shift = fmaf(lam, D, reg2);               // damping + regulariser, added to the pivot at pivot time
           int k = 0;
           auto pivot_steps = [&](auto chunks_tag, int stop_live) {
@@ -1288,14 +1348,12 @@ struct Solver {
             pivot_steps(ChunkTag<8>{}, 24); pivot_steps(ChunkTag<6>{}, 16); pivot_steps(ChunkTag<4>{}, 8); pivot_steps(ChunkTag<2>{}, -1);
           } else if constexpr (HN == 16) {
             pivot_steps(ChunkTag<4>{}, 12); pivot_steps(ChunkTag<3>{}, 8); pivot_steps(ChunkTag<2>{}, 4); pivot_steps(ChunkTag<1>{}, -1);
-          } else if constexpr (HN == 8) {
-            pivot_steps(ChunkTag<2>{}, 4); pivot_steps(ChunkTag<1>{}, -1);
           } else {
-            pivot_steps(ChunkTag<HN / 4>{}, -1);
+            static_assert(HN == 16 || HN == 32, "dense groups are 16 or 32 lanes");
           }
         }
         // back substitution: L^T delta = y (column oriented, transposed copy read conflict free)
-        for (int k = (AR ? 0 : bw) - 1; k >= 0; --k) {
+        for (int k = (dense ? bw : 0) - 1; k >= 0; --k) {
           const int pk = cb + k;
           const float xk = gshfl<G>(y * myinv, pk);
           if (l == pk) y = xk;
@@ -1312,7 +1370,7 @@ struct Solver {
 #pragma unroll
             for (int j = 0; j < HN; ++j) {
               if (AR ? (j < 8 ? j < ar_maxw : j - 8 < ar_t) : j < bw) {
-                const int i = AR ? (j < 8 ? (ar_fb + j < NP ? ar_fb + j : NP - 1) : j - 8) : cb + j;
+                const int i = AR ? (j < 8 ? (ar_fb + j < NP ? ar_fb + j : NP - 1) : j - 8) : (BW > 0 ? (l & ~(BW - 1)) : cb) + j;
                 const float4 ai = at_a(i);
                 const float4 ti_ = at_t(i);
                 const bool up = (anc >> i) & 1u;
@@ -1322,7 +1380,8 @@ struct Solver {
                 const bool mine = !AR || (j < 8 ? j < ar_fw : true);
                 const float v = mine ? (up ? vu : (dn ? vd : 0.f)) : 0.f;
                 // same column bookkeeping as the freeze pass: frozen rows / columns stay zero (identity)
-                const int cj = AR ? (j < 8 ? (j < ar_fw ? ar_fb + j : -1) : (j - 8 < ar_t ? j - 8 : -1)) : cb + j;
+                // (block mode: the window base from the lane index refresh() unpacked, as in the factorisation)
+                const int cj = AR ? (j < 8 ? (j < ar_fw ? ar_fb + j : -1) : (j - 8 < ar_t ? j - 8 : -1)) : (BW > 0 ? (l & ~(BW - 1)) : cb) + j;
                 const bool keep = free_ && cj >= 0 && ((fmask >> (cj & 31)) & 1u);
                 if (drop && keep) hbuf[j * NP + l] -= v;
               }
@@ -1343,8 +1402,14 @@ struct Solver {
         if (bad) xn = x;
         if (revert) xn = x_prev;  // (every lane: the variable set that was free during the reverted step may differ)
         const float dx = xn - x;
-        const float step = gmax<G>(fabsf(dx));
-        const float pred = 0.5f * gsum<G>(dx * fmaf(lam * D, dx, -g));
+        // the step's length and the quadratic model's predicted decrease (block mode: after the trial point's FK and cost, so
+        // that they are not held through them; D of this lane's row is formed again from the backup, as the factorisation
+        // forms its rows' shifts, instead of being held through the trials)
+        float step, pred;
+        if constexpr (BW <= 0) {
+          step = gmax<G>(fabsf(dx));
+          pred = 0.5f * gsum<G>(dx * fmaf(lam * D, dx, -g));
+        }
         const float qn = compose_q(xn);
         fk(qn, Rn, pn);
         refresh();
@@ -1354,6 +1419,11 @@ struct Solver {
         if constexpr (BW > 0) world_axis(Rn, an);
         __syncwarp();
         cost(cur ^ 1, xn);
+        if constexpr (BW > 0) {
+          step = gmax<G>(fabsf(dx));
+          const float Dl = fabsf(free_ ? hb()[(l & (BW - 1)) * NP + l] + reg2 : 1.0f) + 1e-6f;
+          pred = 0.5f * gsum<G>(dx * fmaf(lam * Dl, dx, -g));
+        }
         // F(xn) - F(x) summed term by term: every lane differences its own residual / regulariser term (nearby numbers: the
         // subtraction is exact), so the result carries the rounding of the terms -- a few ulp of each -- and of the link
         // positions behind them, not ulp(F)
@@ -1396,7 +1466,8 @@ struct Solver {
             if (verified) bk.clear_stall();
             gn_prev = gn;
             accepted = true;
-            acc_step = step;
+            if constexpr (BW > 0) bk.set_near(step < kNearStep);  // (a bit of the packed bookkeeping instead of a register)
+            else acc_step = step;
             if (revert) {  // back at the previous point: more damping, or the end when this is the second revert in a row
               lam *= kLamUp;
               bk.inc_rejects();
@@ -1421,7 +1492,7 @@ struct Solver {
           if (bk.exact()) lam = prm.lambda0;  // retry this point with the majoriser model
           else bk.set_done(true);             // no descent direction left at fp32 resolution
         }
-        bk.set_exact(accepted && acc_step < kNearStep);
+        bk.set_exact(accepted && (BW > 0 ? bk.near() : acc_step < kNearStep));
         bk.inc_iters();
         if (bk.iters() >= prm.max_iters && !bk.done()) { bk.set_done(true); bk.flag(DEXR_STATUS_MAXITER); }
       }
