@@ -19,6 +19,8 @@ STATUS_MAXITER = 1 << 24
 STATUS_NONFINITE = 1 << 25
 STATUS_NOT_PD = 1 << 26
 STATUS_MISSING = 1 << 27
+STATUS_PENDING = 1 << 28
+FIXED_LAG_MAX = 4095
 
 _f, _i, _u = C.c_float, C.c_int32, C.c_uint32
 
@@ -139,6 +141,19 @@ class DexrSmoothVjp(C.Structure):
     ]
 
 
+class DexrFixedLag(C.Structure):
+    """Mirror of `dexr_fixed_lag_t`: inputs, caller-owned state and outputs of one fixed-lag smoothing call
+    (`dexr_fixed_lag_step`)."""
+
+    _fields_ = [
+        ("keypoints", C.c_void_p), ("fixed_qpos", C.c_void_p), ("last_qpos", C.c_void_p), ("projected", C.c_void_p),
+        ("window_keypoints", C.c_void_p), ("window_fixed_qpos", C.c_void_p), ("window_qpos", C.c_void_p),
+        ("window_len", C.c_void_p), ("qpos_out", C.c_void_p), ("robot_qpos_out", C.c_void_p), ("status_out", C.c_void_p),
+        ("flush_qpos_out", C.c_void_p), ("flush_robot_qpos_out", C.c_void_p), ("flush_count_out", C.c_void_p),
+        ("lag", _i), ("smooth_weight", _f), ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t),
+    ]
+
+
 class DexrGroup(C.Structure):
     """Mirror of `dexr_group_t`: one (robot, batch) group of a mixed-robot launch."""
 
@@ -162,7 +177,7 @@ EXPORTS = [
     "dexr_sequences_tape_sizeof", "dexr_solve_sequences_tape", "dexr_sequences_vjp_sizeof", "dexr_solve_sequences_vjp",
     "dexr_jacobian_sizeof", "dexr_solve_jacobian", "dexr_solve_sequences_packed", "dexr_solve_sequences_packed_vjp",
     "dexr_smooth_sizeof", "dexr_smooth_workspace_bytes", "dexr_smooth_sequences_packed", "dexr_smooth_vjp_sizeof",
-    "dexr_smooth_sequences_packed_vjp",
+    "dexr_smooth_sequences_packed_vjp", "dexr_fixed_lag_sizeof", "dexr_fixed_lag_workspace_bytes", "dexr_fixed_lag_step",
 ]
 
 _LIB = None
@@ -283,6 +298,17 @@ def load():
                                                          C.c_void_p, C.c_int64, C.c_int64, C.c_void_p]
     elif not os.environ.get("DEXR_LIBRARY"):
         raise DexrError(f"{path} does not export dexr_smooth_vjp_sizeof: rebuild it "
+                        "(python -m dex_retargeting_b200.build --force)")
+    if hasattr(lib, "dexr_fixed_lag_sizeof"):
+        lib.dexr_fixed_lag_sizeof.restype = C.c_size_t
+        if lib.dexr_fixed_lag_sizeof() != C.sizeof(DexrFixedLag):
+            raise DexrError("dexr_fixed_lag_t layout mismatch between library and binding (stale DEXR_LIBRARY?)")
+        lib.dexr_fixed_lag_workspace_bytes.argtypes = [C.c_void_p, C.c_int64, C.c_int32]
+        lib.dexr_fixed_lag_workspace_bytes.restype = C.c_size_t
+        lib.dexr_fixed_lag_step.argtypes = [C.c_void_p, C.POINTER(DexrParams), C.POINTER(DexrFixedLag), C.c_int64,
+                                            C.c_int64, C.c_void_p]
+    elif not os.environ.get("DEXR_LIBRARY"):
+        raise DexrError(f"{path} does not export dexr_fixed_lag_sizeof: rebuild it "
                         "(python -m dex_retargeting_b200.build --force)")
     # (an older A/B library named by DEXR_LIBRARY reads a prefix of the buffer structs -- fields are only ever appended -- so
     # the single-robot entry points still work with it; dexr_solve_frames_multi, whose groups embed the struct, does not)

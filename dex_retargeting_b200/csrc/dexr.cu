@@ -543,6 +543,60 @@ __global__ void __launch_bounds__(kEvalWarps * 32, G == 16 ? 2 : 1) dexr_smooth_
     smooth_vjp_packed_stream(sv, a.io, a.dm, pk, i, lane < G);
 }
 
+// fixed-lag smoothing of live streams: dexr_smooth_kernel's launch shape and stream slots, K ticks of one stream per warp
+// (fixed_lag_tick; a 16-lane warp's second group idles)
+struct FixedLagArgs {
+  const dexr_table_t* table;
+  dexr_params_t prm;  // norm_delta holds the smoothing weight w
+  dexr_fixed_lag_t io;
+  int32_t* wstatus;  // the status words of the workspace (after the smoother's S (L+1) frames)
+  long long S;
+  int K;
+  int flush;
+  Dims dm;
+  int scratch_off;
+  int pos_off;  // shared memory: each warp's loop state, 2 long longs
+};
+
+template <int G>
+__global__ void __launch_bounds__(kEvalWarps * 32, G == 16 ? 2 : 1) dexr_fixed_lag_kernel(const FixedLagArgs a) {
+  load_shared_table(*reinterpret_cast<SharedTable*>(dsmem), a.table);
+  __syncthreads();
+  constexpr int GPW = 32 / G;
+  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
+  const int lane = threadIdx.x & 31;
+  const int gid = warp * GPW + lane / G;
+  Solver<G, 0> sv;
+  sv.init(a.table, a.dm, (uint32_t)(a.scratch_off + gid * VjpScratch<G>::kFloats * 4), a.prm, lane);
+  // the streams dealt as dexr_smooth_kernel deals them.  One loop over (stream, tick) pairs, one tick per iteration: a tick
+  // loop nested in the stream loop holds the smoother's loop invariants in registers through every tick.  The loop state
+  // (stream, tick) lives in shared memory, read by fixed_lag_tick where it needs it, so that none of it is held in a
+  // register across the window solve (the 16-lane kernel spills otherwise).
+  volatile long long* const pos = reinterpret_cast<volatile long long*>(dsmem + a.pos_off) + 2 * warp;
+  const long long first = (long long)warp * gridDim.x + blockIdx.x;
+  if (a.K > 0) {
+    if (lane == 0) {
+      pos[0] = first;
+      pos[1] = 0;
+    }
+    __syncwarp();
+    while (pos[0] < a.S) {
+      fixed_lag_tick(sv, a.io, a.dm, a.prm, a.wstatus, a.K, pos, lane < G);
+      if (lane == 0) {
+        if (pos[1] + 1 < a.K) {
+          pos[1] = pos[1] + 1;
+        } else {
+          pos[1] = 0;
+          pos[0] = pos[0] + (long long)gridDim.x * kEvalWarps;
+        }
+      }
+      __syncwarp();
+    }
+  }
+  if (a.flush)
+    for (long long s = first; s < a.S; s += (long long)gridDim.x * kEvalWarps) fixed_lag_flush(sv, a.io, a.dm, a.prm, s, lane < G);
+}
+
 // ------------------------------------------------------------------------------------------------
 // keypoint pre-processing (single_hand_detector.py:100-103, 130-158): one thread per frame for the 3x3 frame,
 // tile staged through shared memory so that global loads / stores are coalesced 16-byte accesses
@@ -1631,6 +1685,58 @@ extern "C" int dexr_smooth_sequences_packed_vjp(const dexr_robot_t* robot, const
   const PackedLayout pk{offsets, num_streams, num_frames};
   return eval_lanes(r->host) == 16 ? launch_smooth_vjp<16>(r, params, io, pk, stream)
                                    : launch_smooth_vjp<32>(r, params, io, pk, stream);
+}
+
+// dexr_fixed_lag_step: launch_smooth's CTA and occupancy rule.
+template <int G>
+static int launch_fixed_lag(dexr_robot* r, const dexr_params_t* prm, const dexr_fixed_lag_t* io, long long S, int K,
+                            cudaStream_t stream) {
+  FixedLagArgs a{};
+  a.table = r->table_dev;
+  a.prm = *prm;
+  if (!(io->smooth_weight < 0.f)) a.prm.norm_delta = io->smooth_weight;
+  a.io = *io;
+  a.S = S;
+  a.K = K;
+  a.flush = io->flush_count_out != nullptr;
+  a.wstatus = fixed_lag_status_words<G>(*io, S);
+  a.dm = make_dims(r->host);
+  a.scratch_off = round_up((int)sizeof(SharedTable), 16);
+  constexpr int GPW = 32 / G;
+  a.pos_off = round_up(a.scratch_off + kEvalWarps * GPW * VjpScratch<G>::kFloats * 4, 16);
+  const int smem = a.pos_off + kEvalWarps * 2 * (int)sizeof(long long);
+  auto kern = dexr_fixed_lag_kernel<G>;
+  CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  int per_sm = 1;
+  if (int e = eval_ctas_per_sm(kern, smem, &per_sm)) return e;
+  const int grid = (int)std::min<long long>(S, (long long)r->num_sms * per_sm);
+  kern<<<grid, kEvalWarps * 32, smem, stream>>>(a);
+  CUDA_TRY(cudaGetLastError());
+  {
+    std::lock_guard<std::mutex> lk(r->info_mu);
+    r->last = dexr_launch_info_t{grid, kEvalWarps * 32, smem, 0, G, kEvalWarps, r->last.kernels_launched + 1};
+  }
+  return 0;
+}
+
+extern "C" size_t dexr_fixed_lag_sizeof(void) { return sizeof(dexr_fixed_lag_t); }
+
+extern "C" size_t dexr_fixed_lag_workspace_bytes(const dexr_robot_t* robot, int64_t num_streams, int32_t lag) {
+  return robot ? fixed_lag_workspace_bytes(robot->host, num_streams, lag) : 0;
+}
+
+extern "C" int dexr_fixed_lag_step(const dexr_robot_t* robot, const dexr_params_t* params, const dexr_fixed_lag_t* io,
+                                   int64_t num_streams, int64_t num_ticks, void* cuda_stream) {
+  if (!robot || !params || !io) return fail(DEXR_E_INVALID, "dexr_fixed_lag_step: null argument");
+  if (const char* msg = fixed_lag_io_error(robot->host, *io, *params, num_streams, num_ticks))
+    return fail(DEXR_E_INVALID, "%s", msg);
+  if (int e = check_params(params)) return e;
+  if (num_streams == 0 || (num_ticks == 0 && !io->flush_count_out)) return 0;
+  DEVICE_SCOPE(robot->device);
+  dexr_robot* r = const_cast<dexr_robot*>(robot);
+  cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
+  return eval_lanes(r->host) == 16 ? launch_fixed_lag<16>(r, params, io, num_streams, (int)num_ticks, stream)
+                                   : launch_fixed_lag<32>(r, params, io, num_streams, (int)num_ticks, stream);
 }
 
 extern "C" {

@@ -3148,4 +3148,184 @@ __device__ __forceinline__ void smooth_vjp_packed_stream(Solver<G, 0>& sv, const
   __syncwarp();
 }
 
+// ------------------------------------------------------------------------------------------------
+// fixed-lag smoothing of live streams (dexr_fixed_lag_step): each tick runs smooth_packed_stream on a window of the last
+// L+1 frames held in the caller's state (see dexr.h for the semantics)
+// ------------------------------------------------------------------------------------------------
+// Bytes of workspace a call on S streams of lag L needs (dexr_fixed_lag_workspace_bytes): the smoother's for S (L+1) frames,
+// then S (L+1) int32 status words (the window solve's, read back for the emitted frame).
+inline size_t fixed_lag_workspace_bytes(const dexr_table_t& t, long long S, long long lag) {
+  if (S <= 0 || lag < 0 || lag > DEXR_FIXED_LAG_MAX) return 0;
+  const long long frames = S * (lag + 1);
+  return smooth_workspace_bytes(t, frames) + (size_t)frames * sizeof(int32_t);
+}
+
+// Where the status words of a G-lane call's workspace start.
+template <int G>
+inline int32_t* fixed_lag_status_words(const dexr_fixed_lag_t& io, long long S) {
+  return reinterpret_cast<int32_t*>(static_cast<float*>(io.workspace) + S * (io.lag + 1) * SmoothWs<G>::kFloats);
+}
+
+// The argument checks of dexr_fixed_lag_step: nullptr, or what is wrong.  Host code shared by the library and the host
+// emulation.  The per-tick inputs and outputs are required only when there are ticks.
+inline const char* fixed_lag_io_error(const dexr_table_t& t, const dexr_fixed_lag_t& io, const dexr_params_t& prm,
+                                      long long S, long long K) {
+  if (S < 0 || K < 0 || K > INT32_MAX) return "bad sizes: num_streams and num_ticks must be >= 0, num_ticks <= INT32_MAX";
+  if (io.lag < 0 || io.lag > DEXR_FIXED_LAG_MAX) return "lag must be in 0..4095";
+  if (S > INT32_MAX / ((long long)io.lag + 1)) return "num_streams * (lag + 1) must be <= INT32_MAX";
+  if (prm.preprocess != 0) return "raw landmarks are not smoothed: params.preprocess must be 0 (pre-process the keypoints first)";
+  if (!io.last_qpos || !io.window_keypoints || !io.window_qpos || !io.window_len)
+    return "last_qpos, window_keypoints, window_qpos and window_len are required";
+  if (K > 0 && (!io.keypoints || !io.qpos_out)) return "keypoints and qpos_out are required";
+  if (t.len_proj > 0 && !io.projected) return "the robot has DexPilot flags but projected is NULL";
+  if (t.n_fixed > 0 && (!io.window_fixed_qpos || (K > 0 && !io.fixed_qpos)))
+    return "the robot has fixed joints but window_fixed_qpos or fixed_qpos is NULL";
+  if (!(io.smooth_weight < 0.f) && !(io.smooth_weight >= 0.f && io.smooth_weight <= 3.0e38f))
+    return "smooth_weight must be finite (< 0: params.norm_delta)";
+  if (S > 0 && (!io.workspace || io.workspace_bytes < fixed_lag_workspace_bytes(t, S, io.lag)))
+    return "workspace smaller than dexr_fixed_lag_workspace_bytes(robot, num_streams, lag)";
+  return nullptr;
+}
+
+// Advances the committed DexPilot flags `flags` (nullptr: none) by one step of the hysteresis recurrence with the frame at
+// `kp`: prepare_targets' flag update alone, so the flags are those the smoother's walk holds after that frame (it reads only
+// the human vectors).  Lanes below len_proj own one flag each; the second-stage flags read the first stage's by shuffles.
+template <int G>
+__device__ __forceinline__ void fixed_lag_advance_flags(const Solver<G, 0>& sv, const Dims& dm, const dexr_params_t& prm,
+                                                        const float* kp, uint8_t* flags, bool live) {
+  if (flags == nullptr || dm.loss != DEXR_LOSS_DEXPILOT) return;  // (uniform)
+  const SharedTable& st = Solver<G, 0>::ST();
+  const int l = sv.l, len_s1 = dm.len_s1, len_proj = dm.len_proj;
+  float tx = 0.f, ty = 0.f, tz = 0.f;
+  if (live && l < dm.n_res) {
+    const int ht = st.res_ht[l], ho = st.res_ho[l];
+    tx = kp[3 * ht]; ty = kp[3 * ht + 1]; tz = kp[3 * ht + 2];
+    if (ho >= 0) { tx -= kp[3 * ho]; ty -= kp[3 * ho + 1]; tz -= kp[3 * ho + 2]; }
+  }
+  const float dist = sqrtf(fmaf(tx, tx, fmaf(ty, ty, tz * tz)));
+  int flag = 0;
+  if (l < len_s1) {
+    flag = live ? flags[l] : 0;
+    if (dist < prm.project_dist) flag = 1;
+    if (dist > prm.escape_dist) flag = 0;
+  }
+  const int k2 = l - len_s1;
+  const bool is_s2 = (l >= len_s1) && (l < len_proj);
+  const int so = is_s2 ? st.s2_origin[k2] : 0, sk = is_s2 ? st.s2_task[k2] : 0;
+  const int fo = gshfl_i<G>(flag, so), fk_ = gshfl_i<G>(flag, sk);
+  if (is_s2) flag = (fo && fk_ && dist <= 0.03f) ? 1 : 0;
+  if (live && l < len_proj) flags[l] = (uint8_t)flag;
+  __syncwarp();
+}
+
+// The frame at window slot j of stream s: writes its qpos (var lanes) and scatter + mimic (joint lanes) to row `row` of
+// qpos_out / robot_qpos_out, NaN when `emit` is false; robot_qpos as the smoother's output composes it.  Returns x.
+template <int G>
+__device__ __forceinline__ float fixed_lag_emit(Solver<G, 0>& sv, const dexr_fixed_lag_t& io, const Dims& dm, long long s,
+                                                int j, bool emit, bool live, float* qpos_out, float* robot_qpos_out,
+                                                long long row) {
+  const int l = sv.l, W1 = io.lag + 1;
+  const int fixedi = Solver<G, 0>::ST().fixed_index[l];
+  const long long slot = s * W1 + j;
+  const bool rd = live && emit;
+  const float x = (rd && sv.var >= 0) ? io.window_qpos[slot * dm.n_var + sv.var] : 0.f;
+  sv.qfix = (rd && fixedi >= 0) ? io.window_fixed_qpos[slot * dm.n_fixed + fixedi] : 0.f;
+  const float q = sv.compose_q(x);
+  const float nan = __int_as_float(0x7fc00000);
+  if (live) {
+    if (qpos_out && sv.var >= 0) qpos_out[row * dm.n_var + sv.var] = emit ? x : nan;
+    if (robot_qpos_out && l < dm.dof) robot_qpos_out[row * dm.dof + l] = emit ? q : nan;
+  }
+  return x;
+}
+
+// One tick of dexr_fixed_lag_step: tick pos[1] of stream pos[0] (< S).  `pos` is the caller's loop state, read again after
+// the window solve: no index of the driver stays in a register across the smoother, which uses every register the 16-lane
+// kernel has (128); window_len is stored before the solve (the count includes the incoming frame from the append on) and
+// read back after it for the same reason.  `owner`: this group runs the stream (the kernel gives a 16-lane warp's second
+// group none: it walks the same ticks with every read and write off, so that the warp's shuffles stay converged; it reads
+// window_len too).  `wstatus`: the status words after the smoother's part of the workspace.  Between a lane's global
+// writes and another lane's reads, __syncwarp.
+template <int G>
+__device__ __forceinline__ void fixed_lag_tick(Solver<G, 0>& sv, const dexr_fixed_lag_t& io, const Dims& dm,
+                                               const dexr_params_t& prm, int32_t* wstatus, int K,
+                                               const volatile long long* pos, bool owner) {
+  constexpr int KP = 3 * DEXR_NUM_KEYPOINTS;
+  const int l = sv.l, n = dm.n_var, nf = dm.n_fixed, L = io.lag, W1 = L + 1;
+  const bool isvar = sv.var >= 0;
+  {  // 1. append the frame at slot h
+    const long long s = pos[0], fin = s * K + pos[1];
+    const int h0 = io.window_len[s];
+    const int h = h0 < 0 ? 0 : (h0 > L ? L : h0);  // (a count outside 0..L reads as the nearest bound)
+    const long long wh = s * W1 + h;
+    const int fixedi = Solver<G, 0>::ST().fixed_index[l];
+    __syncwarp();  // (every lane has read window_len)
+    if (owner) {
+      for (int e = l; e < KP; e += G) io.window_keypoints[wh * KP + e] = io.keypoints[fin * KP + e];
+      if (fixedi >= 0) io.window_fixed_qpos[wh * nf + fixedi] = io.fixed_qpos[fin * nf + fixedi];
+      if (isvar) io.window_qpos[wh * n + sv.var] = h > 0 ? io.window_qpos[(wh - 1) * n + sv.var] : io.last_qpos[s * n + sv.var];
+      if (l == 0) io.window_len[s] = h + 1;
+    }
+    __syncwarp();
+  }
+  {  // 2. the window solve: the smoother on packed stream s of the window arrays, frames s (L+1) .. s (L+1) + h
+    const long long s = pos[0];
+    dexr_smooth_t sio{};
+    sio.keypoints = io.window_keypoints;
+    sio.fixed_qpos = io.window_fixed_qpos;
+    sio.last_qpos = io.last_qpos;
+    sio.projected = io.projected;
+    sio.qpos_init = io.window_qpos;
+    sio.qpos_out = io.window_qpos;
+    sio.status_out = wstatus;
+    sio.workspace = io.workspace;
+    smooth_packed_stream(sv, sio, dm, prm, PackedStream{s, s * W1, io.window_len[s]}, owner, static_cast<float*>(io.workspace));
+  }
+  // 3. emit slot 0 and commit it, or emit nothing
+  const long long s = pos[0], fin = s * K + pos[1], w0 = s * W1;
+  const bool full = static_cast<const volatile int32_t*>(io.window_len)[s] == W1;
+  const float x = fixed_lag_emit(sv, io, dm, s, 0, full, owner, io.qpos_out, io.robot_qpos_out, fin);
+  if (owner && l == 0 && io.status_out) io.status_out[fin] = full ? wstatus[w0] : DEXR_STATUS_PENDING;
+  if (full) {
+    if (owner && isvar) io.last_qpos[s * n + sv.var] = x;
+    fixed_lag_advance_flags(sv, dm, prm, io.window_keypoints + w0 * KP,
+                            dm.len_proj > 0 ? io.projected + s * dm.len_proj : nullptr, owner);
+    const int fixedi = Solver<G, 0>::ST().fixed_index[l];
+    if (owner) {  // shift the window down by one (each lane moves the entries it owns)
+      for (int j = 0; j < L; ++j) {
+        for (int e = l; e < KP; e += G) io.window_keypoints[(w0 + j) * KP + e] = io.window_keypoints[(w0 + j + 1) * KP + e];
+        if (fixedi >= 0) io.window_fixed_qpos[(w0 + j) * nf + fixedi] = io.window_fixed_qpos[(w0 + j + 1) * nf + fixedi];
+        if (isvar) io.window_qpos[(w0 + j) * n + sv.var] = io.window_qpos[(w0 + j + 1) * n + sv.var];
+      }
+      if (l == 0) io.window_len[s] = L;
+    }
+  }
+  __syncwarp();
+}
+
+// The flush of stream s (< S) of dexr_fixed_lag_step: the held frames as the last solve left them, in order; the last becomes
+// the anchor, the flags advance through them and the window empties.  `owner` as in fixed_lag_tick.
+template <int G>
+__device__ __forceinline__ void fixed_lag_flush(Solver<G, 0>& sv, const dexr_fixed_lag_t& io, const Dims& dm,
+                                                const dexr_params_t& prm, long long s, bool owner) {
+  const int l = sv.l, L = io.lag, W1 = L + 1;
+  const int h0 = io.window_len[s];
+  const int h = h0 < 0 ? 0 : (h0 > L ? L : h0);
+  uint8_t* const flags = dm.len_proj > 0 ? io.projected + s * dm.len_proj : nullptr;
+  for (int j = 0; j < L; ++j) {
+    const bool held = j < h;
+    const float x = fixed_lag_emit(sv, io, dm, s, j, held, owner, io.flush_qpos_out, io.flush_robot_qpos_out, s * L + j);
+    if (held) {
+      if (owner && sv.var >= 0) io.last_qpos[s * dm.n_var + sv.var] = x;
+      fixed_lag_advance_flags(sv, dm, prm, io.window_keypoints + (s * W1 + j) * (3 * DEXR_NUM_KEYPOINTS), flags, owner);
+    }
+  }
+  __syncwarp();  // (every lane has read window_len)
+  if (owner && l == 0) {
+    io.flush_count_out[s] = h;
+    io.window_len[s] = 0;
+  }
+  __syncwarp();
+}
+
 }  // namespace dexr

@@ -14,7 +14,9 @@ With a `SequenceTape` the same launch also records every frame's unfiltered solu
 `retarget_packed_sequences()` / `retarget_packed_sequences_vjp()` do the same for streams of different lengths laid end to
 end (`PackedStreams`, the cu_seqlens layout): recorded clips of any length in one launch, no padding.
 `smooth_packed_sequences()` solves every frame of each packed clip jointly (`dexr_smooth_sequences_packed`): the offline
-trajectory, with no lag and with dropped frames filled in.
+trajectory, with no lag and with dropped frames filled in.  `retarget_fixed_lag()` brings it to live streams
+(`dexr_fixed_lag_step`, `FixedLagState`): each new frame re-solves the last L+1 frames jointly and emits the frame L ticks
+back.
 """
 from __future__ import annotations
 
@@ -71,6 +73,52 @@ class StreamState:
         if st.damping is None:
             st.damping = torch.zeros((S,), dtype=torch.float32, device=st.last_qpos.device)
         return st
+
+
+@dataclass
+class FixedLagState:
+    """Device-resident state of S live streams smoothed with a fixed lag L (`SeqRetargeting.retarget_fixed_lag`, the
+    `dexr_fixed_lag_t` state): the anchor and DexPilot flags after the last committed frame and a window of up to L frames
+    received but not yet committed.  Resumable / checkpointable as `StreamState`."""
+
+    lag: int
+    last_qpos: "torch.Tensor"          # [S, opt_dof] float32, the last committed frame (a fresh stream: the warm start)
+    projected: Optional["torch.Tensor"]  # [S, len_proj] uint8 (DexPilot) or None
+    window_keypoints: "torch.Tensor"   # [S, L+1, 21, 3] float32
+    window_fixed_qpos: Optional["torch.Tensor"]  # [S, L+1, n_fixed] float32, or None without fixed joints
+    window_qpos: "torch.Tensor"        # [S, L+1, opt_dof] float32
+    window_len: "torch.Tensor"         # [S] int32, frames held (0..L)
+
+    _FIELDS = ("last_qpos", "projected", "window_keypoints", "window_fixed_qpos", "window_qpos", "window_len")
+
+    def state_dict(self) -> dict:
+        """Host copies of every tensor (None stays None) and the lag: a run resumed from it continues bit-identically."""
+        d = {k: (None if getattr(self, k) is None else getattr(self, k).detach().cpu().clone()) for k in self._FIELDS}
+        d["lag"] = int(self.lag)
+        return d
+
+    @classmethod
+    def from_state_dict(cls, state: dict, device=None) -> "FixedLagState":
+        """Inverse of `state_dict`: copies of its tensors on `device`."""
+        import torch
+
+        missing = [k for k in ("lag", "last_qpos", "window_keypoints", "window_qpos", "window_len") if state.get(k) is None]
+        if missing:
+            raise ValueError(f"fixed-lag state checkpoint lacks {missing}")
+        S, lag = int(state["last_qpos"].shape[0]), int(state["lag"])
+        for k in cls._FIELDS[1:]:
+            t = state.get(k)
+            if t is not None and int(t.shape[0]) != S:
+                raise ValueError(f"fixed-lag state checkpoint: {k} holds {int(t.shape[0])} streams, last_qpos {S}")
+        for k in ("window_keypoints", "window_fixed_qpos", "window_qpos"):
+            t = state.get(k)
+            if t is not None and int(t.shape[1]) != lag + 1:
+                raise ValueError(f"fixed-lag state checkpoint: {k} holds {int(t.shape[1])} frames, lag {lag} needs {lag + 1}")
+
+        def put(t):  # (a copy: the restored state never aliases the checkpoint)
+            return None if t is None else torch.as_tensor(t).to(device if device is not None else t.device, copy=True).contiguous()
+
+        return cls(lag=lag, **{k: put(state.get(k)) for k in cls._FIELDS})
 
 
 @dataclass
@@ -710,3 +758,118 @@ class SeqRetargeting:
                                                          C.c_void_p(s.cuda_stream)), "dexr_smooth_sequences_packed_vjp")
         ws.record_stream(s)
         return g_kp, g_fixed, g_last
+
+    def make_fixed_lag_state(self, num_streams: int, lag: int) -> FixedLagState:
+        """Initial state of S fresh live streams smoothed with lag L (`retarget_fixed_lag`): the anchor at the mid-range warm
+        start (as `make_stream_state`; `warm_start_batch` applies to `last_qpos`), no DexPilot projection, an empty window."""
+        import torch
+
+        lag = int(lag)
+        if not 0 <= lag <= N.FIXED_LAG_MAX:
+            raise ValueError(f"lag must be in 0..{N.FIXED_LAG_MAX}, got {lag}")
+        opt = self.optimizer
+        base = self.make_stream_state(num_streams)
+        dev = base.last_qpos.device
+        nf = len(opt.idx_pin2fixed)
+        return FixedLagState(
+            lag=lag, last_qpos=base.last_qpos, projected=base.projected,
+            window_keypoints=torch.zeros((num_streams, lag + 1, N.NUM_KEYPOINTS, 3), dtype=torch.float32, device=dev),
+            window_fixed_qpos=(torch.zeros((num_streams, lag + 1, nf), dtype=torch.float32, device=dev) if nf else None),
+            window_qpos=torch.zeros((num_streams, lag + 1, opt.opt_dof), dtype=torch.float32, device=dev),
+            window_len=torch.zeros((num_streams,), dtype=torch.int32, device=dev))
+
+    def _fixed_lag_call(self, state: FixedLagState, K: int, fill, smooth_weight, stream):
+        """One `dexr_fixed_lag_step` call on `state` with K ticks; `fill(io, chk)` sets the per-call buffers."""
+        import torch
+
+        opt = self.optimizer
+        eng = opt.engine()
+        dev = torch.device("cuda", eng.device)
+        chk = _checker(dev)
+        S, L = int(state.last_qpos.shape[0]), int(state.lag)
+        n, nf = opt.opt_dof, len(opt.idx_pin2fixed)
+        io = N.DexrFixedLag()
+        io.lag = L
+        io.last_qpos = chk(state.last_qpos, (S, n), torch.float32, "state.last_qpos")
+        len_proj = opt._objective_spec().len_proj
+        if len_proj:
+            if state.projected is None:
+                raise ValueError("DexPilot streams need state.projected")
+            io.projected = chk(state.projected, (S, len_proj), torch.uint8, "state.projected")
+        io.window_keypoints = chk(state.window_keypoints, (S, L + 1, N.NUM_KEYPOINTS, 3), torch.float32,
+                                  "state.window_keypoints")
+        if nf:
+            if state.window_fixed_qpos is None:
+                raise ValueError(f"Optimizer has {nf} fixed joints but state.window_fixed_qpos is None")
+            io.window_fixed_qpos = chk(state.window_fixed_qpos, (S, L + 1, nf), torch.float32, "state.window_fixed_qpos")
+        io.window_qpos = chk(state.window_qpos, (S, L + 1, n), torch.float32, "state.window_qpos")
+        io.window_len = chk(state.window_len, (S,), torch.int32, "state.window_len")
+        io.smooth_weight = -1.0 if smooth_weight is None else float(smooth_weight)
+        fill(io, chk)
+        nbytes = int(eng.lib.dexr_fixed_lag_workspace_bytes(eng.handle, S, L))
+        ws = torch.empty((max(nbytes, 4),), dtype=torch.uint8, device=dev)
+        io.workspace, io.workspace_bytes = ws.data_ptr(), nbytes
+        s = stream if stream is not None else torch.cuda.current_stream(dev)
+        p = opt.params(clip_init=True, lp_alpha=self.low_pass_alpha)
+        N.check(eng.lib.dexr_fixed_lag_step(eng.handle, C.byref(p), C.byref(io), S, K, C.c_void_p(s.cuda_stream)),
+                "dexr_fixed_lag_step")
+        ws.record_stream(s)
+
+    def retarget_fixed_lag(self, keypoints, state: FixedLagState, *, fixed_qpos=None, smooth_weight=None, out=None,
+                           qpos_out=None, status_out=None, stream=None):
+        """Fixed-lag smoothing of S live streams (`dexr_fixed_lag_step`, one launch): each of the K new frames per stream
+        (keypoints [S,K,21,3], wrist-centred; fixed_qpos [S,K,n_fixed]) re-solves the last L+1 frames of its stream jointly
+        with the offline smoother (`smooth_packed_sequences`, anchored at the last committed frame, w = smooth_weight or
+        norm_delta) and emits the frame L ticks back.  Until a stream's window holds L+1 frames its ticks emit NaN with
+        STATUS_PENDING.  L = 0 is the causal problem; a dropped detection (NaN keypoints) is interpolated from both sides
+        (STATUS_MISSING).  `state` (`make_fixed_lag_state`) is updated in place.  Returns (robot_qpos [S,K,dof] (scatter +
+        mimic, no low-pass filter), qpos [S,K,opt_dof], status [S,K] int32), into `out` / `qpos_out` / `status_out` when
+        given.  Allocates its workspace on the device; nothing is synchronised."""
+        import torch
+
+        opt = self.optimizer
+        if keypoints.dim() != 4 or tuple(keypoints.shape[2:]) != (N.NUM_KEYPOINTS, 3):
+            raise ValueError(f"keypoints must have shape [S,K,21,3], got {tuple(keypoints.shape)}")
+        S, K = int(keypoints.shape[0]), int(keypoints.shape[1])
+        n, dof, nf = opt.opt_dof, opt.robot.dof, len(opt.idx_pin2fixed)
+        dev = state.last_qpos.device
+        qpos = torch.empty((S, K, n), dtype=torch.float32, device=dev) if qpos_out is None else qpos_out
+        if out is None:
+            out = torch.empty((S, K, dof), dtype=torch.float32, device=dev)
+        if status_out is None:
+            status_out = torch.empty((S, K), dtype=torch.int32, device=dev)
+
+        def fill(io, chk):
+            io.keypoints = chk(keypoints, (S, K, N.NUM_KEYPOINTS, 3), torch.float32, "keypoints")
+            if nf:
+                if fixed_qpos is None:
+                    raise ValueError(f"Optimizer has {nf} fixed joints but no fixed_qpos is given")
+                io.fixed_qpos = chk(fixed_qpos, (S, K, nf), torch.float32, "fixed_qpos")
+            io.qpos_out = chk(qpos, (S, K, n), torch.float32, "qpos_out")
+            io.robot_qpos_out = chk(out, (S, K, dof), torch.float32, "out")
+            io.status_out = chk(status_out, (S, K), torch.int32, "status_out")
+
+        self._fixed_lag_call(state, K, fill, smooth_weight, stream)
+        return out, qpos, status_out
+
+    def flush_fixed_lag(self, state: FixedLagState, *, out=None, qpos_out=None, count_out=None, stream=None):
+        """End S fixed-lag streams: emit the frames each still holds, in order, as the last tick's joint solve left them (no
+        new solve), commit the last of them as the anchor and empty the windows.  Returns (robot_qpos [S,L,dof], qpos
+        [S,L,opt_dof], count [S] int32), into `out` / `qpos_out` / `count_out` when given: stream s's rows 0..count[s]-1 are
+        its held frames, the rest NaN."""
+        import torch
+
+        opt = self.optimizer
+        S, L = int(state.last_qpos.shape[0]), int(state.lag)
+        dev = state.last_qpos.device
+        qpos = torch.empty((S, L, opt.opt_dof), dtype=torch.float32, device=dev) if qpos_out is None else qpos_out
+        rq = torch.empty((S, L, opt.robot.dof), dtype=torch.float32, device=dev) if out is None else out
+        count = torch.empty((S,), dtype=torch.int32, device=dev) if count_out is None else count_out
+
+        def fill(io, chk):
+            io.flush_qpos_out = chk(qpos, (S, L, opt.opt_dof), torch.float32, "qpos_out")
+            io.flush_robot_qpos_out = chk(rq, (S, L, opt.robot.dof), torch.float32, "out")
+            io.flush_count_out = chk(count, (S,), torch.int32, "count_out")
+
+        self._fixed_lag_call(state, 0, fill, None, stream)
+        return rq, qpos, count

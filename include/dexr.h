@@ -521,6 +521,66 @@ int dexr_smooth_sequences_packed_vjp(const dexr_robot_t* robot, const dexr_param
                                      const int64_t* offsets /* device [S+1] */, int64_t num_streams, int64_t num_frames,
                                      void* cuda_stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Fixed-lag smoothing of live streams: every new frame re-solves the last L+1 frames of its stream jointly with the offline
+ * smoother and emits the frame L ticks back.  A stream trades a fixed delay of L frames for the smoother's answer on its
+ * window: no jitter from the one-sided anchor of the causal solve, dropped detections filled in from both sides.
+ * State per stream s (caller-owned, in/out; the lag L is fixed for the life of the state):
+ *   last_qpos[s]            the anchor a: the last committed frame's solution (a fresh stream: the warm start, as
+ *                           dexr_sequences_t.last_qpos);
+ *   projected[s]            the DexPilot flags after the last committed frame (a fresh stream: all false);
+ *   window_len[s]           h in 0..L, the frames held but not yet committed, in time order at slots 0..h-1 of
+ *                           window_keypoints / window_fixed_qpos / window_qpos (slot L takes the incoming frame).
+ * A tick (num_ticks of them per call, stream s reading keypoints[s,k] at tick k):
+ *   1. append the frame at slot h; window_qpos[h] starts at window_qpos[h-1] (h = 0: last_qpos);
+ *   2. solve: exactly dexr_smooth_sequences_packed on the h+1 window frames (keypoints = window_keypoints, fixed_qpos =
+ *      window_fixed_qpos, qpos_init = qpos_out = window_qpos, last_qpos = the anchor, projected = the committed flags,
+ *      w = smooth_weight (< 0: params.norm_delta); params.tol, lambda0 and max_iters per tick);
+ *   3. if h + 1 = L + 1: emit slot 0 (qpos_out, robot_qpos_out = its scatter + mimic, status_out = the window solve's status
+ *      word of that frame, DEXR_STATUS_MAXITER and DEXR_STATUS_MISSING included), commit it (last_qpos = window_qpos[0],
+ *      projected advanced by one step of the hysteresis recurrence with its keypoints: the smoother's own walk) and shift
+ *      the window down by one.  Otherwise window_len = h + 1 and the tick emits NaN with status DEXR_STATUS_PENDING.
+ * Flush (flush_count_out non-NULL, after the ticks): the held frames are emitted in order as the last tick's joint solve left
+ *   them (rows 0..h-1 of flush_*_out, NaN after; flush_count_out[s] = h), the last one becomes the anchor, the flags advance
+ *   through them and window_len = 0.  No new solve: (x_1..x_L) of the window's minimiser minimises it with x_0 fixed.  After
+ *   a flush a stream fed T frames has emitted exactly T non-pending frames.
+ * So L = 0 is the causal problem (each tick minimises L_t(x) + w |x - clip(x_{t-1})|^2), and L >= T - 1 followed by a flush
+ *   is the offline smoother on the whole clip from the same anchor.  A dropped detection (a NaN keypoint or fixed joint) is
+ *   the smoother's missing frame: interpolated inside the window once later frames arrive, emitted with
+ *   DEXR_STATUS_MISSING.  A stream whose state is non-finite emits DEXR_STATUS_NONFINITE (the smoother's rule for a
+ *   non-finite start) until the caller resets it.  No low-pass filter (params.lp_alpha is ignored), no carried damping.
+ *   A window_len outside 0..L reads as the nearest bound.  Raw landmarks (params.preprocess != 0) are refused.
+ *   `workspace`: at least dexr_fixed_lag_workspace_bytes(robot, num_streams, lag) bytes (DEXR_E_INVALID below): the
+ *   smoother's workspace for S (L+1) frames followed by S (L+1) int32 status words.  num_ticks == 0 without a flush does
+ *   nothing.  Asynchronous on `cuda_stream`, allocates nothing.  All pointers are DEVICE pointers.
+ * ------------------------------------------------------------------------------------------- */
+#define DEXR_STATUS_PENDING (1 << 28) /* fixed lag: the tick filled the window and emitted nothing (qpos NaN) */
+#define DEXR_FIXED_LAG_MAX 4095       /* the largest lag */
+typedef struct dexr_fixed_lag {
+  const float* keypoints;      /* [S,K,21,3] new frames, wrist-centred (params.preprocess must be 0)                   */
+  const float* fixed_qpos;     /* [S,K,n_fixed] or NULL when n_fixed == 0                                             */
+  float* last_qpos;            /* [S,n_var] in/out anchor: the last committed frame / the warm start                  */
+  uint8_t* projected;          /* [S,len_proj] in/out flags after the last committed frame, or NULL                   */
+  float* window_keypoints;     /* [S,L+1,21,3] in/out                                                                  */
+  float* window_fixed_qpos;    /* [S,L+1,n_fixed] in/out or NULL                                                       */
+  float* window_qpos;          /* [S,L+1,n_var] in/out                                                                 */
+  int32_t* window_len;         /* [S] in/out, 0..L                                                                     */
+  float* qpos_out;             /* [S,K,n_var] frame emitted at each tick (NaN while PENDING)                           */
+  float* robot_qpos_out;       /* [S,K,dof] or NULL                                                                    */
+  int32_t* status_out;         /* [S,K] or NULL                                                                        */
+  float* flush_qpos_out;       /* [S,L,n_var] or NULL                                                                  */
+  float* flush_robot_qpos_out; /* [S,L,dof] or NULL                                                                    */
+  int32_t* flush_count_out;    /* [S] or NULL: non-NULL = flush after the K ticks                                      */
+  int32_t lag;
+  float smooth_weight;         /* < 0: params.norm_delta                                                               */
+  void* workspace;             /* >= dexr_fixed_lag_workspace_bytes(robot, S, lag) bytes                               */
+  size_t workspace_bytes;
+} dexr_fixed_lag_t;
+size_t dexr_fixed_lag_sizeof(void);
+size_t dexr_fixed_lag_workspace_bytes(const dexr_robot_t* robot, int64_t num_streams, int32_t lag);
+int dexr_fixed_lag_step(const dexr_robot_t* robot, const dexr_params_t* params, const dexr_fixed_lag_t* io,
+                        int64_t num_streams, int64_t num_ticks, void* cuda_stream);
+
 #ifdef __cplusplus
 }
 #endif
