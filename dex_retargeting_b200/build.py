@@ -30,6 +30,7 @@ def find_nvcc() -> str:
 VARIANTS = {
     "fastsincos": ["-DDEXR_EXP_FASTSINCOS"],
     "multi_calls": ["-DDEXR_EXP_MULTI_CALLS"],
+    "timeline": ["-DDEXR_EXP_TIMELINE"],  # frames kernel event timeline for tools/frames_timeline.py
 }
 
 

@@ -19,19 +19,81 @@ namespace dexr {
 // ------------------------------------------------------------------------------------------------
 // kernel arguments
 // ------------------------------------------------------------------------------------------------
+// The tile queue of one frames launch (FrameArgs::queue): tiles handed out beyond every CTA's first tile, and the CTAs
+// that are done with it.  The launch's last CTA zeroes it again.  Library-owned slots, one launch at a time per slot
+// (dexr_robot::queue_dev).
+struct QueueSlot {
+  unsigned int next, done;
+};
+
+constexpr int kMaxLevels = 6;
+
 struct FrameArgs {
   const dexr_table_t* table;
   dexr_params_t prm;
   dexr_frames_t io;
   long long B;
-  int T;          // frames per tile (multiple of 4)
-  int ntiles;
+  int T;          // frames per full tile (multiple of 4, except the exact one-round tiles)
+  int ntiles;     // full tiles: the static schedule's count
+  int stages;     // input ring depth
+  int min_chunk;  // queue: smallest tile handed out as the queue runs dry (= T: tiles never shrink)
+  QueueSlot* queue;  // nullptr: static striding (tiles first_tile, first_tile + gridDim.x, ...)
+  int n_levels;      // queue schedule after the grid's first tiles: lv_tiles[j] tiles of lv_size[j] frames, j = 0, 1, ...
+  int lv_tiles[kMaxLevels], lv_size[kMaxLevels];
+  unsigned long long* timeline;  // DEXR_EXP_TIMELINE builds: event buffer (frames_timeline.py); otherwise unused
   int use_bulk;   // inputs 16-byte aligned -> cp.async.bulk for full tiles
   int in_row;     // floats per frame of the kp/ref input (63 or 3m)
   Dims dm;
   int off_in, off_last, off_fixed, stage_bytes;  // ring stage layout (bytes)
   int ring_off, bar_off, scratch_off;            // dynamic smem layout (bytes)
 };
+
+// Experiment build DEXR_EXP_TIMELINE: the frames kernel records when each of its warps waits and works, into a buffer the
+// caller passes with dexr_exp_timeline() (tools/frames_timeline.py reads it).  Layout, 64-bit words: an event count per
+// (CTA, warp) for kTlCtas x 32 warps, then kTlEvents events of 4 words per (CTA, warp): {kind << 32 | x, y, t0, t1} with
+// %globaltimer nanoseconds.  Kinds: 0 warp span (entry, exit), 1 consumer frame claim (x = first frame, y = frames),
+// 2 consumer wait on a stage (x = tile's first frame, y = frames), 3 producer wait for a free stage, 4 producer tile claim
+// (x = first frame, y = frames), 5 consumer prologue (entry to table loaded and solver set up).  The default build records nothing.
+constexpr int kTlCtas = 256, kTlEvents = 128;
+struct Timeline {
+#ifdef DEXR_EXP_TIMELINE
+  unsigned long long* w = nullptr;
+  unsigned long long* cnt = nullptr;
+  int n = 0;
+  __device__ __forceinline__ Timeline(unsigned long long* buf, int warp) {
+    if (buf && blockIdx.x < kTlCtas && threadIdx.x % 32 == 0) {
+      const int slot = blockIdx.x * 32 + warp;
+      cnt = buf + slot;
+      w = buf + kTlCtas * 32 + (size_t)slot * kTlEvents * 4;
+    }
+  }
+  __device__ __forceinline__ static unsigned long long now() {
+    unsigned long long t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    return t;
+  }
+  __device__ __forceinline__ void event(int kind, long long x, long long y, unsigned long long t0, unsigned long long t1) {
+    if (w && n < kTlEvents) {
+      w[4 * n] = ((unsigned long long)kind << 32) | (unsigned int)x;
+      w[4 * n + 1] = (unsigned long long)y;
+      w[4 * n + 2] = t0;
+      w[4 * n + 3] = t1;
+      ++n;
+    }
+  }
+  __device__ __forceinline__ void close() {
+    if (cnt) *cnt = (unsigned long long)n;
+  }
+#else
+  __device__ __forceinline__ Timeline(unsigned long long*, int) {}
+  __device__ __forceinline__ static unsigned long long now() { return 0; }
+  __device__ __forceinline__ void event(int, long long, long long, unsigned long long, unsigned long long) {}
+  __device__ __forceinline__ void close() {}
+#endif
+};
+#ifdef DEXR_EXP_TIMELINE
+static unsigned long long* g_timeline = nullptr;  // set by dexr_exp_timeline(), passed to every frames launch
+#endif
 
 struct SeqArgs {
   const dexr_table_t* table;
@@ -49,45 +111,68 @@ struct SeqArgs {
 // ------------------------------------------------------------------------------------------------
 // independent frames: producer warp (TMA ring) + NCW consumer warps
 // ------------------------------------------------------------------------------------------------
-// One robot group, executed by one CTA: the tiles `first_tile, first_tile + gridDim.x, ...` of the group's batch.  Both the
-// single-robot kernel and the mixed-robot kernel (several groups back to back inside one launch) run this body; it starts
-// and ends with a CTA-wide barrier, so it can be called repeatedly with different tables / template parameters.
+// One robot group, executed by one CTA.  Its first tile is `first_tile`; after that it takes the tiles
+// `first_tile + gridDim.x, first_tile + 2 gridDim.x, ...` (static striding, a.queue == nullptr), or claims tiles from the
+// launch's queue (a.queue), which hands out the frames beyond the grid's first tiles in tiles that shrink as it runs dry.
+// The producer writes each tile's first frame and size next to its stage; a size of 0 tells the consumers that the group
+// is done.  Both the single-robot kernel and the mixed-robot kernel (several groups back to back inside one launch) run
+// this body; it starts with a CTA-wide barrier and leaves every barrier phase complete, so it can be called repeatedly with
+// different tables / template parameters.
 template <int G, int BW, int NCW>
 __device__ __forceinline__ void frames_group(const FrameArgs& a, int first_tile) {
   unsigned char* const smem = dsmem;
   SharedTable* st = reinterpret_cast<SharedTable*>(smem);
   unsigned char* ring = smem + a.ring_off;
+  const int S = a.stages;
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + a.bar_off);
-  uint64_t* empty = full + 2;
-  int* next = reinterpret_cast<int*>(empty + 2);
-
-  __syncthreads();  // (mixed launches: every warp is done with the previous group's table, ring and barriers)
-  load_shared_table(*st, a.table, pass_slot_width<BW>());
-  if (threadIdx.x == 0) {
-    mbar_init(&full[0], 1);
-    mbar_init(&full[1], 1);
-    mbar_init(&empty[0], NCW);
-    mbar_init(&empty[1], NCW);
-    next[0] = 0;
-    next[1] = 0;
-    mbar_fence_init();
-  }
-  __syncthreads();
+  uint64_t* empty = full + S;
+  long long* tile_f0 = reinterpret_cast<long long*>(empty + S);
+  int* next = reinterpret_cast<int*>(tile_f0 + S);
+  int* tile_n = next + S;
 
   // warp-uniform by construction: tells the compiler that the role split below never splits a warp
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
   const int lane = threadIdx.x & 31;
+  Timeline tl(a.timeline, warp);
+  const unsigned long long t_entry = Timeline::now();
+
+  __syncthreads();  // (mixed launches: every warp is done with the previous group's table, ring and barriers)
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < S; ++s) {
+      mbar_init(&full[s], 1);
+      mbar_init(&empty[s], NCW);
+    }
+    mbar_fence_init();
+  }
+  __syncthreads();
+
   const bool by_kp = a.io.keypoints != nullptr;
   const float* g_in = by_kp ? a.io.keypoints : a.io.ref_value;
 
   if (warp == NCW) {
     // ===================== producer: stage tiles HBM -> shared memory =====================
-    int it = 0;
-    for (int tile = first_tile; tile < a.ntiles; tile += gridDim.x, ++it) {
-      const int stage = it & 1;
-      if (it >= 2) mbar_wait(&empty[stage], ((it >> 1) - 1) & 1);
-      const long long f0 = (long long)tile * a.T;
-      const int count = (int)min((long long)a.T, a.B - f0);
+    // frames the grid's first tiles cover: the queue hands out the rest
+    const long long head = min(a.B, (long long)gridDim.x * a.T);
+    long long f0 = (long long)first_tile * a.T;
+    int count = (int)max(0LL, min((long long)a.T, a.B - f0));
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int it = 0;; ++it) {
+      if (it >= S) {
+        const unsigned long long t0 = Timeline::now();
+        mbar_wait(&empty[stage], phase ^ 1u);
+        tl.event(3, 0, 0, t0, Timeline::now());
+      }
+      if (lane == 0) {
+        tile_f0[stage] = f0;
+        tile_n[stage] = count;
+        next[stage] = 0;
+      }
+      if (count == 0) {  // end of the group: every consumer reads the size 0 and leaves
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&full[stage]);
+        break;
+      }
       unsigned char* sb = ring + stage * a.stage_bytes;
       float* s_in = reinterpret_cast<float*>(sb + a.off_in);
       float* s_last = reinterpret_cast<float*>(sb + a.off_last);
@@ -95,7 +180,6 @@ __device__ __forceinline__ void frames_group(const FrameArgs& a, int first_tile)
       const float* gi = g_in + f0 * a.in_row;
       const float* gl = a.io.last_qpos + f0 * a.dm.n_var;
       const float* gf = a.dm.n_fixed > 0 ? a.io.fixed_qpos + f0 * a.dm.n_fixed : nullptr;
-      if (lane == 0) next[stage] = 0;
       if (a.use_bulk && (count & 3) == 0) {
         if (lane == 0) {
           const uint32_t b_in = (uint32_t)count * a.in_row * 4u;
@@ -115,20 +199,74 @@ __device__ __forceinline__ void frames_group(const FrameArgs& a, int first_tile)
         if (lane == 0) mbar_arrive(&full[stage]);
       }
       __syncwarp();
+      if (++stage == S) {
+        stage = 0;
+        phase ^= 1u;
+      }
+      // the next tile
+      if (!a.queue) {
+        f0 += (long long)gridDim.x * a.T;
+        count = (int)max(0LL, min((long long)a.T, a.B - f0));
+      } else {
+        // One atomicAdd per claim (a compare-and-swap loop on the frame count stalls once every CTA claims at the same
+        // time, as they do while the queue runs dry): the k-th claim of the launch gets the k-th tile of a fixed schedule
+        // (FrameArgs::lv_*), full tiles first, then tiles that shrink level by level (see plan_queue).
+        if (lane == 0) {
+          const unsigned long long t0 = Timeline::now();
+          int k = (int)atomicAdd(&a.queue->next, 1u);
+          long long f = head;
+          count = 0;
+          for (int j = 0; j < a.n_levels; ++j) {
+            if (k < a.lv_tiles[j]) {
+              f0 = f + (long long)k * a.lv_size[j];
+              count = (int)min((long long)a.lv_size[j], a.B - f0);
+              break;
+            }
+            k -= a.lv_tiles[j];
+            f += (long long)a.lv_tiles[j] * a.lv_size[j];
+          }
+          if (count) tl.event(4, f0, count, t0, Timeline::now());
+        }
+        f0 = __shfl_sync(0xffffffffu, f0, 0);
+        count = __shfl_sync(0xffffffffu, count, 0);
+      }
+    }
+    if (a.queue && lane == 0) {
+      // This CTA's last claim found the queue empty.  The last CTA to get here knows that no CTA of the launch will read
+      // the queue again and zeroes it for the next launch that takes this slot.
+      __threadfence();
+      if (atomicAdd(&a.queue->done, 1u) == gridDim.x - 1) {
+        a.queue->next = 0;
+        a.queue->done = 0;
+      }
     }
   } else {
     // ===================== consumers: one frame per group of G lanes =========================
+    // The consumers load the table while the producer's first tiles are in flight, and wait for each other only (named
+    // barrier 1).  Every array of the table has at most 32 entries, so threads of warp 0 copy all of it and the producer
+    // warp has no part in load_shared_table.
+    load_shared_table(*st, a.table, pass_slot_width<BW>());
+    asm volatile("bar.sync 1, %0;" ::"r"(NCW * 32) : "memory");
     constexpr int GPW = 32 / G;
     const int gid = warp * GPW + (lane / G);
     Solver<G, BW> sv;
     sv.init(a.table, a.dm, (uint32_t)(a.scratch_off + gid * Scratch<G, BW>::kFloats * 4), a.prm, lane);
+    tl.event(5, 0, 0, t_entry, Timeline::now());
 
-    int it = 0;
-    for (int tile = first_tile; tile < a.ntiles; tile += gridDim.x, ++it) {
-      const int stage = it & 1;
-      mbar_wait(&full[stage], (it >> 1) & 1);
-      const long long f0 = (long long)tile * a.T;
-      const int count = (int)min((long long)a.T, a.B - f0);
+    for (int it = 0;; ++it) {
+      const int stage = it % S;
+      const unsigned long long t_wait = Timeline::now();
+      mbar_wait(&full[stage], (uint32_t)(it / S) & 1u);
+      // the stage's first frame and size are reread from shared memory where they are used: nothing lives in registers
+      // across solve_frame that the static schedule did not keep there
+      const volatile long long* v_f0 = tile_f0 + stage;
+      const volatile int* v_n = tile_n + stage;
+      tl.event(2, *v_f0, *v_n, t_wait, Timeline::now());
+      if (*v_n == 0) {  // the group is done; arriving keeps the stage's barrier phases complete for the next group
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty[stage]);
+        break;
+      }
       const unsigned char* sb = ring + stage * a.stage_bytes;
       const float* s_in = reinterpret_cast<const float*>(sb + a.off_in);
       const float* s_last = reinterpret_cast<const float*>(sb + a.off_last);
@@ -137,23 +275,28 @@ __device__ __forceinline__ void frames_group(const FrameArgs& a, int first_tile)
         int base = 0;
         if (lane == 0) base = atomicAdd(&next[stage], GPW);
         base = __shfl_sync(0xffffffffu, base, 0);
+        const int count = *v_n;
         if (base >= count) break;
         const int idx = base + (lane / G);
         const bool active = idx < count;
         const int ci = active ? idx : base;
-        const long long f = f0 + ci;
+        const long long f = *v_f0 + ci;
         FrameInputs in;
         in.kp = by_kp ? s_in + ci * a.in_row : nullptr;
         in.ref = by_kp ? nullptr : s_in + ci * a.in_row;
         in.last = s_last + ci * a.dm.n_var;
         in.fixed = s_fixed + ci * a.dm.n_fixed;
         in.projected = a.io.projected ? a.io.projected + f * a.dm.len_proj : nullptr;
+        const unsigned long long t0 = Timeline::now();
         solve_frame(sv, in, a.io, a.dm, f, active);
+        tl.event(1, f - ci + base, min(GPW, *v_n - base), t0, Timeline::now());
       }
       __syncwarp();
       if (lane == 0) mbar_arrive(&empty[stage]);
     }
   }
+  tl.event(0, blockIdx.x, warp, t_entry, Timeline::now());
+  tl.close();
 }
 
 template <int G, int BW, int NCW>
@@ -716,6 +859,8 @@ struct DeviceGuard {
     if (_e != cudaSuccess) return fail(DEXR_E_CUDA, "%s failed: %s", #expr, cudaGetErrorString(_e)); \
   } while (0)
 
+constexpr int kQueueSlots = 16;
+
 struct dexr_robot {
   int device = 0;
   int num_sms = 0;
@@ -728,9 +873,33 @@ struct dexr_robot {
   cudaStream_t streams[2] = {nullptr, nullptr};
   void* stage_dev[2] = {nullptr, nullptr};
   size_t stage_bytes = 0;
+  int smem_optin = 0;  // dynamic shared memory a CTA may opt in to
+  // Tile queues of the frames kernel: kQueueSlots zeroed slots, each with the event recorded behind the last launch that
+  // used it.  A launch takes a slot whose event has completed: that launch has ended, and its last CTA left the slot
+  // zeroed.  So two launches that can overlap (two streams, or this robot in two groups of one mixed call) never share a
+  // slot, with no memset or extra kernel per call.  When every slot is in use, the launch waits on its stream for the
+  // next slot's event (work enqueued earlier: this cannot deadlock).  queue_mu covers the choice and the launch.
+  QueueSlot* queue_dev = nullptr;
+  cudaEvent_t queue_ev[kQueueSlots] = {};
+  int queue_next = 0;
+  std::mutex queue_mu;
 };
 
 static int frames_max_tile(int lanes) { return lanes == 16 ? 64 : 32; }  // frames per ring stage (shared memory budget)
+
+// Input ring depth of the frames kernel: 4 stages (measured: DESIGN.md 3.1); DEXR_FRAMES_STAGES=2|3|4 (read per call)
+// overrides for A/B runs.  fill_frame_args takes fewer where a CTA's shared memory would not fit.
+static int frames_stages() {
+  const char* e = getenv("DEXR_FRAMES_STAGES");
+  const int s = e ? atoi(e) : 0;
+  return s >= 2 && s <= 4 ? s : 4;
+}
+
+// DEXR_FRAMES_QUEUE=0 (read per call) hands the tiles out by static striding instead of the grid-wide queue, for A/B runs.
+static bool frames_queue_enabled() {
+  const char* e = getenv("DEXR_FRAMES_QUEUE");
+  return !(e && atoi(e) == 0);
+}
 constexpr int kSeqNW = 8;       // warps per CTA (sequences kernel)
 
 static int validate_table(const dexr_table_t* t) {
@@ -828,6 +997,16 @@ static int finish_create(dexr_robot* r, dexr_robot_t** out) {
     return fail(DEXR_E_NODEVICE, "device %d is sm_%d%d; libdexr is built for sm_90a (H100) only", device, prop.major, prop.minor);
   }
   r->num_sms = prop.multiProcessorCount;
+  r->smem_optin = (int)prop.sharedMemPerBlockOptin;
+  // the frames kernel's tile queue slots start zeroed (the synchronise: before any launch on any stream can read them)
+  ce = cudaMalloc(&r->queue_dev, kQueueSlots * sizeof(QueueSlot));
+  if (ce == cudaSuccess) ce = cudaMemset(r->queue_dev, 0, kQueueSlots * sizeof(QueueSlot));
+  if (ce == cudaSuccess) ce = cudaDeviceSynchronize();
+  for (int i = 0; i < kQueueSlots && ce == cudaSuccess; ++i) ce = cudaEventCreateWithFlags(&r->queue_ev[i], cudaEventDisableTiming);
+  if (ce != cudaSuccess) {
+    dexr_robot_destroy(r);
+    return fail(DEXR_E_CUDA, "allocating the frames kernel's tile queues failed: %s", cudaGetErrorString(ce));
+  }
   *out = r;
   return 0;
 }
@@ -916,6 +1095,9 @@ void dexr_robot_destroy(dexr_robot_t* robot) {
     if (robot->streams[i]) cudaStreamDestroy(robot->streams[i]);
     if (robot->stage_dev[i]) cudaFree(robot->stage_dev[i]);
   }
+  for (int i = 0; i < kQueueSlots; ++i)
+    if (robot->queue_ev[i]) cudaEventDestroy(robot->queue_ev[i]);
+  if (robot->queue_dev) cudaFree(robot->queue_dev);
   if (robot->table_dev) cudaFree(robot->table_dev);
   delete robot;
 }
@@ -978,10 +1160,45 @@ static int fill_frame_args(const dexr_robot* r, const dexr_params_t* prm, const 
   a.off_fixed = a.off_last + round_up(T * t.n_var * 4, 16);
   a.stage_bytes = a.off_fixed + round_up(T * std::max(t.n_fixed, 1) * 4, 16);
   a.ring_off = round_up((int)sizeof(SharedTable), 16);
-  a.bar_off = a.ring_off + 2 * a.stage_bytes;
-  a.scratch_off = round_up(a.bar_off + 4 * 8 + 2 * 4, 16);
+  // Ring depth: frames_stages() (4), fewer where the shared memory of the CTA would not fit.  Per stage: the tile, two
+  // barriers and the tile's first frame (8 bytes each), its frame claim counter and its size (4 bytes each).
   constexpr int GPW = 32 / G;
-  return a.scratch_off + NCW * GPW * Scratch<G, BW>::kFloats * 4;
+  const int scratch_bytes = NCW * GPW * Scratch<G, BW>::kFloats * 4;
+  int S = frames_stages();
+  auto layout = [&](int s) {
+    a.stages = s;
+    a.bar_off = a.ring_off + s * a.stage_bytes;
+    a.scratch_off = round_up(a.bar_off + s * 32, 16);
+    return a.scratch_off + scratch_bytes;
+  };
+  while (S > 2 && layout(S) > r->smem_optin) --S;
+  const int smem = layout(S);
+  // the queue's smallest tile: about one round of the CTA's warps over the ring's stages (block 16, 24 warps, 4 stages:
+  // 12 frames); tiles that are not a multiple of 4 (exact one-round tiles) never shrink
+  a.min_chunk = (T & 3) ? T : std::min(T, round_up((kRound + S - 1) / S, 4));
+  return smem;
+}
+
+// The queue's schedule (frames_group): after the grid's first tiles, full tiles while more than stages x grid x (the next
+// size) frames would be left, then tiles of half the size, and so on down to min_chunk.  Sizes are multiples of 4, so
+// every tile's inputs stay 16-byte aligned for the bulk copy; only the batch's ragged end is smaller.  A CTA holds at
+// most `stages` claimed tiles, so near the end what it holds is at most its share of the rest, and the CTAs end within
+// about one smallest tile of each other: guided self-scheduling, with the sizes fixed per launch.
+static void plan_queue(FrameArgs& a, int grid) {
+  long long rest = a.B - (long long)grid * a.T;
+  const long long share = (long long)a.stages * grid;
+  int c = a.T;
+  a.n_levels = 0;
+  while (rest > 0) {
+    const int nc = std::max(a.min_chunk, round_up(c / 2, 4));
+    const bool last = c <= a.min_chunk || a.n_levels == kMaxLevels - 1;
+    const long long n = last ? (rest + c - 1) / c : std::max(0LL, (rest - share * nc) / c);
+    a.lv_size[a.n_levels] = c;
+    a.lv_tiles[a.n_levels] = (int)n;
+    ++a.n_levels;
+    rest -= n * c;
+    c = nc;
+  }
 }
 
 template <int G, int BW, int NCW>
@@ -992,8 +1209,33 @@ static int launch_frames(dexr_robot* r, const dexr_params_t* prm, const dexr_fra
   auto kern = dexr_frames_kernel<G, BW, NCW>;
   CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
   const int grid = std::min(a.ntiles, slots);
-  kern<<<grid, (NCW + 1) * 32, smem, stream>>>(a);
-  CUDA_TRY(cudaGetLastError());
+#ifdef DEXR_EXP_TIMELINE
+  a.timeline = g_timeline;
+#endif
+  if ((long long)grid * a.T >= B || !frames_queue_enabled()) {  // every CTA's first tile covers the batch: no queue
+    kern<<<grid, (NCW + 1) * 32, smem, stream>>>(a);
+    CUDA_TRY(cudaGetLastError());
+  } else {
+    std::lock_guard<std::mutex> lk(r->queue_mu);
+    int slot = -1;
+    for (int k = 0; k < kQueueSlots && slot < 0; ++k) {
+      const int i = (r->queue_next + k) % kQueueSlots;
+      const cudaError_t q = cudaEventQuery(r->queue_ev[i]);
+      if (q == cudaSuccess) slot = i;
+      else if (q == cudaErrorNotReady) cudaGetLastError();  // (not an error: the slot is in use)
+      else return fail(DEXR_E_CUDA, "cudaEventQuery on a tile queue slot failed: %s", cudaGetErrorString(q));
+    }
+    if (slot < 0) {
+      slot = r->queue_next;
+      CUDA_TRY(cudaStreamWaitEvent(stream, r->queue_ev[slot], 0));
+    }
+    r->queue_next = (slot + 1) % kQueueSlots;
+    a.queue = r->queue_dev + slot;
+    plan_queue(a, grid);
+    kern<<<grid, (NCW + 1) * 32, smem, stream>>>(a);
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaEventRecord(r->queue_ev[slot], stream));
+  }
   {
     std::lock_guard<std::mutex> lk(r->info_mu);
     r->last = dexr_launch_info_t{grid, (NCW + 1) * 32, smem, a.T, G, NCW, r->last.kernels_launched + 1};
@@ -1364,6 +1606,15 @@ extern "C" int dexr_solve_frames(const dexr_robot_t* robot, const dexr_params_t*
   cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
   return launch_frames_kind(r, params, io, num_frames, stream);
 }
+
+#ifdef DEXR_EXP_TIMELINE
+// Experiment builds only: the device buffer the frames kernel records its events into from the next launch on (nullptr:
+// none).  Returns the buffer's size in bytes (layout: Timeline).
+extern "C" int64_t dexr_exp_timeline(void* buffer) {
+  g_timeline = static_cast<unsigned long long*>(buffer);
+  return (int64_t)kTlCtas * 32 * (1 + 4 * kTlEvents) * 8;
+}
+#endif
 
 // Launch shape of the sequences kernels for S streams: sets a.spw and a.duo, returns the grid.
 // A stream is serial in time and latency bound, so streams are spread over as many warps and SMs as there are: while one

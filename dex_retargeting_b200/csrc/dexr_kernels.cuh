@@ -24,8 +24,8 @@
 //   * for sequences, SeqRetargeting's clip -> solve -> scatter -> mimic -> low-pass recurrence
 //     (seq_retarget.py:112-134, optimizer_utils.py:7-13) carried in registers across time steps.
 // Inputs of a batch are staged HBM (or pinned host memory, zero-copy) -> shared memory by a producer warp
-// with cp.async.bulk (TMA 1-D) into a two-stage ring guarded by mbarriers; consumer warps claim frames
-// from the ring dynamically.
+// with cp.async.bulk (TMA 1-D) into a ring of up to four stages guarded by mbarriers; the CTAs claim tiles from a
+// grid-wide queue, and consumer warps claim frames from the ring dynamically.
 // No tensor cores: n <= 32 unknowns per frame, the work is FP32 issue / latency bound.
 #pragma once
 
@@ -287,6 +287,9 @@ __device__ inline void load_shared_table(SharedTable& st, const dexr_table_t* __
     st.s2_origin[i] = tb->s2_origin[i];
     st.s2_task[i] = tb->s2_task[i];
   }
+#ifndef DEXR_HOST_EMULATION
+  __syncwarp();  // lanes 0-15 of warp 0 wrote the link and residual arrays that thread 0 reads below
+#endif
   for (int i = threadIdx.x; i < DEXR_MAX_LANES; i += blockDim.x) {
     int cnt = 0;
     for (int k = 0; k < tb->n_links; ++k)
@@ -302,11 +305,16 @@ __device__ inline void load_shared_table(SharedTable& st, const dexr_table_t* __
     st.fixed_index[i] = tb->fixed_index[i];
     st.group_count[i] = tb->group_count[i];
     if (i == 0) {  // most links any single lane carries (1 for every shipped hand)
+      // Thread 0 runs this part alone while the CTA waits: it counts and schedules from the shared copies of the link
+      // parents, masks and residual links, not through chains of dependent global loads (links on the same lane as link
+      // k, for every link k on a lane: parents are < dof <= 32, -1 for the world).
+      const int nl = tb->n_links;
       int mx = 0;
-      for (int c = 0; c < DEXR_MAX_LANES; ++c) {
+      DEXR_ROLL for (int k = 0; k < nl; ++k) {
+        const int pk = __float_as_int(st.link_off[k].w);
         int n = 0;
-        for (int k = 0; k < tb->n_links; ++k) n += (tb->link_parent[k] == c);
-        mx = n > mx ? n : mx;
+        DEXR_ROLL for (int j = 0; j < nl; ++j) n += (__float_as_int(st.link_off[j].w) == pk);
+        if (pk >= 0) mx = n > mx ? n : mx;
       }
       st.own_rounds = mx > DEXR_MAX_LINKS_PER_LANE ? DEXR_MAX_LINKS_PER_LANE : mx;
       {
@@ -317,8 +325,8 @@ __device__ inline void load_shared_table(SharedTable& st, const dexr_table_t* __
           for (int sl = 0; sl < nslot; ++sl) st.pass_res[r][sl] = -1;
         int np = 0;
         for (int k = 0; k < tb->n_res; ++k) {
-          const uint32_t msk = tb->link_anc_mask[tb->res_task[k]] |
-                               (tb->res_origin[k] >= 0 ? tb->link_anc_mask[tb->res_origin[k]] : 0u);
+          const int rt = st.res_task[k], ro = st.res_origin[k];
+          const uint32_t msk = st.link_anc[rt] | (ro >= 0 ? st.link_anc[ro] : 0u);
           uint32_t sm = 0u;  // slots this residual touches; one that touches no joint rides in slot 0 (it still counts
           for (int sl = 0; sl < nslot && sl * gr < 32; ++sl)  // for the residual maximum)
             if ((msk >> (sl * gr)) & ((1u << gr) - 1u)) sm |= 1u << sl;
