@@ -53,7 +53,8 @@ struct FrameArgs {
 // (CTA, warp) for kTlCtas x 32 warps, then kTlEvents events of 4 words per (CTA, warp): {kind << 32 | x, y, t0, t1} with
 // %globaltimer nanoseconds.  Kinds: 0 warp span (entry, exit), 1 consumer frame claim (x = first frame, y = frames),
 // 2 consumer wait on a stage (x = tile's first frame, y = frames), 3 producer wait for a free stage, 4 producer tile claim
-// (x = first frame, y = frames), 5 consumer prologue (entry to table loaded and solver set up).  The default build records nothing.
+// (x = first frame, y = frames), 5 consumer prologue (entry to table loaded and solver set up), 6 consumer warp's totals at its
+// exit (x = outer iterations its solver ran, y = frames it solved).  The default build records nothing.
 constexpr int kTlCtas = 256, kTlEvents = 128;
 struct Timeline {
 #ifdef DEXR_EXP_TIMELINE
@@ -111,6 +112,14 @@ struct SeqArgs {
 // ------------------------------------------------------------------------------------------------
 // independent frames: producer warp (TMA ring) + NCW consumer warps
 // ------------------------------------------------------------------------------------------------
+// Programmatic dependent launch (launch_frames_kernel): the next kernel of the stream may be launched as soon as every CTA
+// of this one has started, so its CTAs take the SMs this launch's CTAs leave and run their set-up while the rest of this
+// launch finishes.  grid_dep_wait() returns once the previous kernel of the stream has completed and its writes are
+// visible; the frames kernel reads nothing the previous kernel may write before it (the robot table is only written by
+// copies, never by a kernel).  Both are no-ops in a kernel not launched that way.
+__device__ __forceinline__ void grid_dep_launch() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
+__device__ __forceinline__ void grid_dep_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+
 // One robot group, executed by one CTA.  Its first tile is `first_tile`; after that it takes the tiles
 // `first_tile + gridDim.x, first_tile + 2 gridDim.x, ...` (static striding, a.queue == nullptr), or claims tiles from the
 // launch's queue (a.queue), which hands out the frames beyond the grid's first tiles in tiles that shrink as it runs dry.
@@ -155,6 +164,7 @@ __device__ __forceinline__ void frames_group(const FrameArgs& a, int first_tile)
     const long long head = min(a.B, (long long)gridDim.x * a.T);
     long long f0 = (long long)first_tile * a.T;
     int count = (int)max(0LL, min((long long)a.T, a.B - f0));
+    grid_dep_wait();  // (the inputs and the queue)
     int stage = 0;
     uint32_t phase = 0;
     for (int it = 0;; ++it) {
@@ -246,6 +256,7 @@ __device__ __forceinline__ void frames_group(const FrameArgs& a, int first_tile)
     // barrier 1).  Every array of the table has at most 32 entries, so threads of warp 0 copy all of it and the producer
     // warp has no part in load_shared_table.
     load_shared_table(*st, a.table, pass_slot_width<BW>());
+    grid_dep_wait();  // (the damping words and every output)
     asm volatile("bar.sync 1, %0;" ::"r"(NCW * 32) : "memory");
     constexpr int GPW = 32 / G;
     const int gid = warp * GPW + (lane / G);
@@ -253,6 +264,7 @@ __device__ __forceinline__ void frames_group(const FrameArgs& a, int first_tile)
     sv.init(a.table, a.dm, (uint32_t)(a.scratch_off + gid * Scratch<G, BW>::kFloats * 4), a.prm, lane);
     tl.event(5, 0, 0, t_entry, Timeline::now());
 
+    long long solved = 0;  // (timeline builds: frames this warp solved)
     for (int it = 0;; ++it) {
       const int stage = it % S;
       const unsigned long long t_wait = Timeline::now();
@@ -290,10 +302,14 @@ __device__ __forceinline__ void frames_group(const FrameArgs& a, int first_tile)
         const unsigned long long t0 = Timeline::now();
         solve_frame(sv, in, a.io, a.dm, f, active);
         tl.event(1, f - ci + base, min(GPW, *v_n - base), t0, Timeline::now());
+#ifdef DEXR_EXP_TIMELINE
+        solved += min(GPW, *v_n - base);
+#endif
       }
       __syncwarp();
       if (lane == 0) mbar_arrive(&empty[stage]);
     }
+    tl.event(6, sv.issued, solved, t_entry, Timeline::now());
   }
   tl.event(0, blockIdx.x, warp, t_entry, Timeline::now());
   tl.close();
@@ -301,6 +317,7 @@ __device__ __forceinline__ void frames_group(const FrameArgs& a, int first_tile)
 
 template <int G, int BW, int NCW>
 __global__ void __launch_bounds__((NCW + 1) * 32, 1) dexr_frames_kernel(const FrameArgs a) {
+  grid_dep_launch();
   frames_group<G, BW, NCW>(a, blockIdx.x);
 }
 
@@ -1173,9 +1190,11 @@ static int fill_frame_args(const dexr_robot* r, const dexr_params_t* prm, const 
   };
   while (S > 2 && layout(S) > r->smem_optin) --S;
   const int smem = layout(S);
-  // the queue's smallest tile: about one round of the CTA's warps over the ring's stages (block 16, 24 warps, 4 stages:
-  // 12 frames); tiles that are not a multiple of 4 (exact one-round tiles) never shrink
-  a.min_chunk = (T & 3) ? T : std::min(T, round_up((kRound + S - 1) / S, 4));
+  // the queue's smallest tile: about two rounds of the CTA's warps over the ring's stages (block 16, 24 warps, 4 stages:
+  // 24 frames).  Every tile costs a claim and a staging, and with smaller tiles the warps wait for stages at the end of
+  // the launch more than the finer split saves (DESIGN.md 3.1).  Tiles that are not a multiple of 4 (exact one-round
+  // tiles) never shrink.
+  a.min_chunk = (T & 3) ? T : std::min(T, round_up((2 * kRound + S - 1) / S, 4));
   return smem;
 }
 
@@ -1201,6 +1220,29 @@ static void plan_queue(FrameArgs& a, int grid) {
   }
 }
 
+// DEXR_FRAMES_PDL=0 (read per call) launches the single-robot frames kernel without programmatic dependent launch, for
+// A/B runs.
+static bool frames_pdl_enabled() {
+  const char* e = getenv("DEXR_FRAMES_PDL");
+  return !(e && atoi(e) == 0);
+}
+
+// The single-robot frames kernel, launched with programmatic stream serialisation (see grid_dep_launch).
+template <class K>
+static cudaError_t launch_frames_kernel(K kern, int grid, int block, int smem, cudaStream_t stream, const FrameArgs& a) {
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(grid);
+  cfg.blockDim = dim3(block);
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = stream;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = frames_pdl_enabled() ? 1 : 0;
+  return cudaLaunchKernelEx(&cfg, kern, a);
+}
+
 template <int G, int BW, int NCW>
 static int launch_frames(dexr_robot* r, const dexr_params_t* prm, const dexr_frames_t* io, long long B, cudaStream_t stream, int slots, int tile) {
   FrameArgs a;
@@ -1213,8 +1255,7 @@ static int launch_frames(dexr_robot* r, const dexr_params_t* prm, const dexr_fra
   a.timeline = g_timeline;
 #endif
   if ((long long)grid * a.T >= B || !frames_queue_enabled()) {  // every CTA's first tile covers the batch: no queue
-    kern<<<grid, (NCW + 1) * 32, smem, stream>>>(a);
-    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(launch_frames_kernel(kern, grid, (NCW + 1) * 32, smem, stream, a));
   } else {
     std::lock_guard<std::mutex> lk(r->queue_mu);
     int slot = -1;
@@ -1232,8 +1273,7 @@ static int launch_frames(dexr_robot* r, const dexr_params_t* prm, const dexr_fra
     r->queue_next = (slot + 1) % kQueueSlots;
     a.queue = r->queue_dev + slot;
     plan_queue(a, grid);
-    kern<<<grid, (NCW + 1) * 32, smem, stream>>>(a);
-    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(launch_frames_kernel(kern, grid, (NCW + 1) * 32, smem, stream, a));
     CUDA_TRY(cudaEventRecord(r->queue_ev[slot], stream));
   }
   {

@@ -500,6 +500,11 @@ struct Solver {
                               // half `duo`: the merged residual passes are dealt alternately to the two halves -- same
                               // instructions, other residuals -- and their partial gradient / Hessian sums are added across the
                               // halves with full-width shuffles.  Everything else runs redundantly in both halves.
+#ifdef DEXR_EXP_TIMELINE
+  long long issued = 0;       // outer iterations this group's warp has run, masked ones included (tools/frames_timeline.py)
+#else
+  static constexpr long long issued = 0;
+#endif
 
   __device__ __forceinline__ static const SharedTable& ST() { return *reinterpret_cast<const SharedTable*>(dsmem); }
 
@@ -849,6 +854,9 @@ struct Solver {
     }
 
     while (gany<32>(!bk.done(), lane)) {
+#ifdef DEXR_EXP_TIMELINE
+      ++issued;
+#endif
       refresh();
       // ======================= gradient + exact Hessian at x ===========================
       float H[HN];

@@ -14,6 +14,11 @@ Allegro, 65 536 frames, warm start sigma 0.05) and of the sigma 0.5 cold start, 
   head_idle       consumer warp-time from the launch's start to each warp's first frame, share
   bound           1 - busy / (consumer warps x launch): the share of the launch that no schedule of the same frames on
                   the same warps could beat (time spent solving frames is fixed; everything else is scheduling)
+  issued_per_frame  outer iterations the consumer warps ran per frame and group: a warp's iteration count times its
+                  groups (32 / lanes per frame) over the frames it solved.  The two frames of a warp run until both are
+                  done, so this is the mean over frame pairs of the larger of the two frames' iteration counts.  A frame
+                  runs one iteration more than its status word counts when it converges (the iteration whose step meets
+                  the tolerance is not counted): compare it with iterations_mean + 1, the frames' own mean.
 
 Schedules (environment switches of the library, read per call): `static<S>` = tiles strided over the CTAs
 (DEXR_FRAMES_QUEUE=0), `queue<S>` = the grid-wide queue with shrinking tail tiles; S = input ring stages
@@ -61,12 +66,14 @@ def decode(buf: np.ndarray, ctas: int, events: int) -> list[dict]:
     return out
 
 
-def analyse(warps: list[dict], ncw: int) -> dict:
+def analyse(warps: list[dict], ncw: int, groups: int = 2) -> dict:
+    """groups: frames a consumer warp solves at a time (32 / lanes per frame)"""
     spans, cta_end = [], {}
     busy = stage_wait = tail = head = 0
     t_start = min(int(w["ev"][w["ev"][:, 0] >> 32 == 0][0, 2]) for w in warps)
     t_end = max(int(w["ev"][w["ev"][:, 0] >> 32 == 0][0, 3]) for w in warps)
     n_cons = 0
+    issued = solved = 0
     for w in warps:
         ev = w["ev"]
         kind = ev[:, 0] >> 32
@@ -77,6 +84,10 @@ def analyse(warps: list[dict], ncw: int) -> dict:
         n_cons += 1
         claims = ev[kind == 1]
         waits = ev[kind == 2]
+        totals = ev[kind == 6]
+        if len(totals):
+            issued += int(totals[0, 0] & 0xFFFFFFFF) * groups
+            solved += int(totals[0, 1])
         busy += int((claims[:, 3] - claims[:, 2]).sum())
         if len(waits) > 1:
             stage_wait += int((waits[1:, 3] - waits[1:, 2]).sum())  # the first wait is the launch's start-up
@@ -99,6 +110,7 @@ def analyse(warps: list[dict], ncw: int) -> dict:
         "tail_idle": tail / total,
         "head_idle": head / total,
         "bound": 1.0 - busy / total,
+        "issued_per_frame": issued / max(solved, 1),
     }
 
 
@@ -143,7 +155,8 @@ for cfg in configs:
             torch.cuda.synchronize()
             lib.dexr_exp_timeline(None)
             info = opt.engine().launch_info()
-            stats.append(analyse(decode(buf.cpu().numpy().view(np.uint64), CTAS, EVENTS), info["consumer_warps"]))
+            stats.append(analyse(decode(buf.cpu().numpy().view(np.uint64), CTAS, EVENTS), info["consumer_warps"],
+                                 32 // info["lanes_per_frame"]))
         med = sorted(stats, key=lambda s: s["launch_us"])[len(stats) // 2]
         med["launch_us_all"] = [round(s["launch_us"], 2) for s in stats]
         med.update(config=cfg, arm=arm, iterations_mean=float((status.cpu().numpy() & 0xffff).mean()),
@@ -178,10 +191,10 @@ def main():
     print(f"\n{info.get('name', '?')}, power limit {info.get('power.limit', '?')}, SM clock {info.get('clocks.sm', '?')} "
           f"(max {info.get('clocks.max.sm', '?')})")
     print(f"{'arm':<11} {'schedule':<8} {'launch us':>9} {'CTA end spread':>18} {'stage wait':>10} {'tail idle':>9} "
-          f"{'head idle':>9} {'bound':>6}")
+          f"{'head idle':>9} {'bound':>6} {'issued/frame':>12} {'iters/frame + 1':>15}")
     for r in recs:
         print(f"{r['arm']:<11} {r['config']:<8} {r['launch_us']:>9.1f} {r['cta_end_spread_us']:>8.1f} us {100 * r['cta_end_spread']:>5.1f} % "
-              f"{100 * r['stage_wait']:>9.1f}% {100 * r['tail_idle']:>8.1f}% {100 * r['head_idle']:>8.1f}% {100 * r['bound']:>5.1f}%")
+              f"{100 * r['stage_wait']:>9.1f}% {100 * r['tail_idle']:>8.1f}% {100 * r['head_idle']:>8.1f}% {100 * r['bound']:>5.1f}% {r['issued_per_frame']:>12.2f} {r['iterations_mean'] + 1:>15.2f}")
 
 
 if __name__ == "__main__":
