@@ -154,6 +154,30 @@ class DexrFixedLag(C.Structure):
     ]
 
 
+class DexrFixedLagTape(C.Structure):
+    """Mirror of `dexr_fixed_lag_tape_t`: what `dexr_fixed_lag_step_tape` records for the backward."""
+
+    _fields_ = [("qpos", C.c_void_p), ("projected", C.c_void_p)]
+
+
+class DexrFixedLagVjp(C.Structure):
+    """Mirror of `dexr_fixed_lag_vjp_t`: buffers of one backpropagation through a fixed-lag call
+    (`dexr_fixed_lag_step_vjp`)."""
+
+    _fields_ = [
+        ("keypoints", C.c_void_p), ("fixed_qpos", C.c_void_p), ("last_qpos", C.c_void_p), ("projected", C.c_void_p),
+        ("window_keypoints", C.c_void_p), ("window_fixed_qpos", C.c_void_p), ("window_qpos", C.c_void_p),
+        ("window_len", C.c_void_p), ("tape", DexrFixedLagTape), ("grad_qpos", C.c_void_p),
+        ("grad_robot_qpos", C.c_void_p), ("grad_flush_qpos", C.c_void_p), ("grad_flush_robot_qpos", C.c_void_p),
+        ("grad_last_qpos_out", C.c_void_p), ("grad_window_qpos_out", C.c_void_p),
+        ("grad_window_keypoints_out", C.c_void_p), ("grad_window_fixed_qpos_out", C.c_void_p),
+        ("grad_keypoints", C.c_void_p), ("grad_fixed_qpos", C.c_void_p), ("grad_last_qpos", C.c_void_p),
+        ("grad_window_keypoints", C.c_void_p), ("grad_window_fixed_qpos", C.c_void_p), ("grad_window_qpos", C.c_void_p),
+        ("status_out", C.c_void_p), ("lag", _i), ("flushed", _i), ("smooth_weight", _f), ("workspace", C.c_void_p),
+        ("workspace_bytes", C.c_size_t),
+    ]
+
+
 class DexrGroup(C.Structure):
     """Mirror of `dexr_group_t`: one (robot, batch) group of a mixed-robot launch."""
 
@@ -178,6 +202,8 @@ EXPORTS = [
     "dexr_jacobian_sizeof", "dexr_solve_jacobian", "dexr_solve_sequences_packed", "dexr_solve_sequences_packed_vjp",
     "dexr_smooth_sizeof", "dexr_smooth_workspace_bytes", "dexr_smooth_sequences_packed", "dexr_smooth_vjp_sizeof",
     "dexr_smooth_sequences_packed_vjp", "dexr_fixed_lag_sizeof", "dexr_fixed_lag_workspace_bytes", "dexr_fixed_lag_step",
+    "dexr_fixed_lag_tape_sizeof", "dexr_fixed_lag_step_tape", "dexr_fixed_lag_vjp_sizeof",
+    "dexr_fixed_lag_vjp_workspace_bytes", "dexr_fixed_lag_step_vjp",
 ]
 
 _LIB = None
@@ -309,6 +335,22 @@ def load():
                                             C.c_int64, C.c_void_p]
     elif not os.environ.get("DEXR_LIBRARY"):
         raise DexrError(f"{path} does not export dexr_fixed_lag_sizeof: rebuild it "
+                        "(python -m dex_retargeting_b200.build --force)")
+    if hasattr(lib, "dexr_fixed_lag_vjp_sizeof"):
+        lib.dexr_fixed_lag_tape_sizeof.restype = C.c_size_t
+        lib.dexr_fixed_lag_vjp_sizeof.restype = C.c_size_t
+        if (lib.dexr_fixed_lag_tape_sizeof() != C.sizeof(DexrFixedLagTape)
+                or lib.dexr_fixed_lag_vjp_sizeof() != C.sizeof(DexrFixedLagVjp)):
+            raise DexrError("dexr_fixed_lag_tape_t / dexr_fixed_lag_vjp_t layout mismatch between library and binding "
+                            "(stale DEXR_LIBRARY?)")
+        lib.dexr_fixed_lag_step_tape.argtypes = [C.c_void_p, C.POINTER(DexrParams), C.POINTER(DexrFixedLag),
+                                                 C.POINTER(DexrFixedLagTape), C.c_int64, C.c_int64, C.c_void_p]
+        lib.dexr_fixed_lag_vjp_workspace_bytes.argtypes = [C.c_void_p, C.c_int64, C.c_int32]
+        lib.dexr_fixed_lag_vjp_workspace_bytes.restype = C.c_size_t
+        lib.dexr_fixed_lag_step_vjp.argtypes = [C.c_void_p, C.POINTER(DexrParams), C.POINTER(DexrFixedLagVjp), C.c_int64,
+                                                C.c_int64, C.c_void_p]
+    elif not os.environ.get("DEXR_LIBRARY"):
+        raise DexrError(f"{path} does not export dexr_fixed_lag_vjp_sizeof: rebuild it "
                         "(python -m dex_retargeting_b200.build --force)")
     # (an older A/B library named by DEXR_LIBRARY reads a prefix of the buffer structs -- fields are only ever appended -- so
     # the single-robot entry points still work with it; dexr_solve_frames_multi, whose groups embed the struct, does not)

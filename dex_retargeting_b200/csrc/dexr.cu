@@ -718,8 +718,10 @@ struct FixedLagArgs {
   int pos_off;  // shared memory: each warp's loop state, 2 long longs
 };
 
-template <int G>
-__global__ void __launch_bounds__(kEvalWarps * 32, G == 16 ? 2 : 1) dexr_fixed_lag_kernel(const FixedLagArgs a) {
+// The body of dexr_fixed_lag_kernel and dexr_fixed_lag_tape_kernel; REC (dexr_fixed_lag_step_tape): fixed_lag_tick's
+// recording into `tape`.
+template <int G, bool REC>
+__device__ __forceinline__ void fixed_lag_kernel_body(const FixedLagArgs& a, const dexr_fixed_lag_tape_t& tape) {
   load_shared_table(*reinterpret_cast<SharedTable*>(dsmem), a.table);
   __syncthreads();
   constexpr int GPW = 32 / G;
@@ -741,7 +743,7 @@ __global__ void __launch_bounds__(kEvalWarps * 32, G == 16 ? 2 : 1) dexr_fixed_l
     }
     __syncwarp();
     while (pos[0] < a.S) {
-      fixed_lag_tick(sv, a.io, a.dm, a.prm, a.wstatus, a.K, pos, lane < G);
+      fixed_lag_tick<G, REC>(sv, a.io, a.dm, a.prm, a.wstatus, a.K, pos, lane < G, tape.qpos, tape.projected);
       if (lane == 0) {
         if (pos[1] + 1 < a.K) {
           pos[1] = pos[1] + 1;
@@ -755,6 +757,81 @@ __global__ void __launch_bounds__(kEvalWarps * 32, G == 16 ? 2 : 1) dexr_fixed_l
   }
   if (a.flush)
     for (long long s = first; s < a.S; s += (long long)gridDim.x * kEvalWarps) fixed_lag_flush(sv, a.io, a.dm, a.prm, s, lane < G);
+}
+
+template <int G>
+__global__ void __launch_bounds__(kEvalWarps * 32, G == 16 ? 2 : 1) dexr_fixed_lag_kernel(const FixedLagArgs a) {
+  fixed_lag_kernel_body<G, false>(a, dexr_fixed_lag_tape_t{nullptr, nullptr});
+}
+
+// dexr_fixed_lag_step_tape: dexr_fixed_lag_kernel with fixed_lag_tick's recording switched on.
+template <int G>
+__global__ void __launch_bounds__(kEvalWarps * 32, G == 16 ? 2 : 1) dexr_fixed_lag_tape_kernel(const FixedLagArgs a,
+                                                                                               const dexr_fixed_lag_tape_t tape) {
+  fixed_lag_kernel_body<G, true>(a, tape);
+}
+
+// backpropagation through fixed-lag smoothing: dexr_smooth_vjp_kernel's launch shape, the streams dealt as
+// dexr_fixed_lag_kernel deals them, a stream's ticks walked in reverse on its warp (a 16-lane warp's second group idles)
+struct FixedLagVjpArgs {
+  const dexr_table_t* table;
+  dexr_params_t prm;  // norm_delta holds the smoothing weight w
+  dexr_fixed_lag_vjp_t io;
+  dexr_smooth_vjp_t wio;  // the window VJP's view of the workspace (fixed_lag_vjp_window_io)
+  PackedLayout wpk;       // its packed layout: stream s's window is packed stream 2 s
+  FixedLagVjpWs ws;
+  long long S;
+  int K;
+  Dims dm;
+  int scratch_off;
+  int pos_off;  // shared memory: each warp's loop state, 2 long longs
+};
+
+template <int G>
+__global__ void __launch_bounds__(kEvalWarps * 32, G == 16 ? 2 : 1) dexr_fixed_lag_vjp_kernel(const FixedLagVjpArgs a) {
+  load_shared_table(*reinterpret_cast<SharedTable*>(dsmem), a.table);
+  __syncthreads();
+  constexpr int GPW = 32 / G;
+  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
+  const int lane = threadIdx.x & 31;
+  const int gid = warp * GPW + lane / G;
+  Solver<G, 0> sv;
+  sv.init(a.table, a.dm, (uint32_t)(a.scratch_off + gid * VjpScratch<G>::kFloats * 4), a.prm, lane);
+  // One loop over (stream, tick) pairs, the ticks of a stream from K-1 down to 0, one per iteration; the loop state lives in
+  // shared memory as in dexr_fixed_lag_kernel, so that none of it is held in a register across the window VJP.  Its address
+  // is recomputed at each use (`pos()`), and the lane read again from threadIdx: held through the window VJP, either is a
+  // register the 16-lane kernel does not have (it spills otherwise).
+  auto pos = [&]() {
+    return reinterpret_cast<volatile long long*>(dsmem + a.pos_off) + 2 * opaque((uint32_t)(threadIdx.x >> 5));
+  };
+  const long long first = (long long)warp * gridDim.x + blockIdx.x;
+  if (a.K == 0) {
+    for (long long s = first; s < a.S; s += (long long)gridDim.x * kEvalWarps)
+      fixed_lag_vjp_begin(sv, a.io, a.ws, a.dm, s, 0, (threadIdx.x & 31) < G);
+    return;
+  }
+  if ((threadIdx.x & 31) == 0) {
+    pos()[0] = first;
+    pos()[1] = a.K - 1;
+  }
+  __syncwarp();
+  while (pos()[0] < a.S) {
+    if (pos()[1] == a.K - 1) fixed_lag_vjp_begin(sv, a.io, a.ws, a.dm, pos()[0], a.K, (threadIdx.x & 31) < G);
+    if (fixed_lag_vjp_rebuild(sv, a.io, a.ws, a.dm, a.K, pos(), (threadIdx.x & 31) < G)) {
+      smooth_vjp_packed_stream(sv, a.wio, a.dm, a.wpk, 2 * pos()[0], (threadIdx.x & 31) < G);
+      fixed_lag_vjp_scatter(sv, a.io, a.ws, a.dm, a.K, pos(), (threadIdx.x & 31) < G);
+    }
+    if ((threadIdx.x & 31) == 0) {
+      volatile long long* const p = pos();
+      if (p[1] > 0) {
+        p[1] = p[1] - 1;
+      } else {
+        p[1] = a.K - 1;
+        p[0] = p[0] + (long long)gridDim.x * kEvalWarps;
+      }
+    }
+    __syncwarp();
+  }
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1981,7 +2058,7 @@ extern "C" int dexr_smooth_sequences_packed_vjp(const dexr_robot_t* robot, const
 // dexr_fixed_lag_step: launch_smooth's CTA and occupancy rule.
 template <int G>
 static int launch_fixed_lag(dexr_robot* r, const dexr_params_t* prm, const dexr_fixed_lag_t* io, long long S, int K,
-                            cudaStream_t stream) {
+                            cudaStream_t stream, const dexr_fixed_lag_tape_t* tape = nullptr) {
   FixedLagArgs a{};
   a.table = r->table_dev;
   a.prm = *prm;
@@ -1997,11 +2074,14 @@ static int launch_fixed_lag(dexr_robot* r, const dexr_params_t* prm, const dexr_
   a.pos_off = round_up(a.scratch_off + kEvalWarps * GPW * VjpScratch<G>::kFloats * 4, 16);
   const int smem = a.pos_off + kEvalWarps * 2 * (int)sizeof(long long);
   auto kern = dexr_fixed_lag_kernel<G>;
+  auto kern_tape = dexr_fixed_lag_tape_kernel<G>;
   CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  if (tape) CUDA_TRY(cudaFuncSetAttribute(kern_tape, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
   int per_sm = 1;
   if (int e = eval_ctas_per_sm(kern, smem, &per_sm)) return e;
   const int grid = (int)std::min<long long>(S, (long long)r->num_sms * per_sm);
-  kern<<<grid, kEvalWarps * 32, smem, stream>>>(a);
+  if (tape) kern_tape<<<grid, kEvalWarps * 32, smem, stream>>>(a, *tape);
+  else kern<<<grid, kEvalWarps * 32, smem, stream>>>(a);
   CUDA_TRY(cudaGetLastError());
   {
     std::lock_guard<std::mutex> lk(r->info_mu);
@@ -2028,6 +2108,79 @@ extern "C" int dexr_fixed_lag_step(const dexr_robot_t* robot, const dexr_params_
   cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
   return eval_lanes(r->host) == 16 ? launch_fixed_lag<16>(r, params, io, num_streams, (int)num_ticks, stream)
                                    : launch_fixed_lag<32>(r, params, io, num_streams, (int)num_ticks, stream);
+}
+
+extern "C" size_t dexr_fixed_lag_tape_sizeof(void) { return sizeof(dexr_fixed_lag_tape_t); }
+
+extern "C" int dexr_fixed_lag_step_tape(const dexr_robot_t* robot, const dexr_params_t* params, const dexr_fixed_lag_t* io,
+                                        const dexr_fixed_lag_tape_t* tape, int64_t num_streams, int64_t num_ticks,
+                                        void* cuda_stream) {
+  if (!robot || !params || !io || !tape) return fail(DEXR_E_INVALID, "dexr_fixed_lag_step_tape: null argument");
+  if (const char* msg = fixed_lag_io_error(robot->host, *io, *params, num_streams, num_ticks))
+    return fail(DEXR_E_INVALID, "%s", msg);
+  if (num_ticks > 0)
+    if (const char* msg = fixed_lag_tape_error(robot->host, tape)) return fail(DEXR_E_INVALID, "%s", msg);
+  if (int e = check_params(params)) return e;
+  if (num_streams == 0 || (num_ticks == 0 && !io->flush_count_out)) return 0;
+  DEVICE_SCOPE(robot->device);
+  dexr_robot* r = const_cast<dexr_robot*>(robot);
+  cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
+  const dexr_fixed_lag_tape_t tp{tape->qpos, robot->host.len_proj > 0 ? tape->projected : nullptr};
+  return eval_lanes(r->host) == 16 ? launch_fixed_lag<16>(r, params, io, num_streams, (int)num_ticks, stream, &tp)
+                                   : launch_fixed_lag<32>(r, params, io, num_streams, (int)num_ticks, stream, &tp);
+}
+
+// dexr_fixed_lag_step_vjp: launch_fixed_lag's CTA and occupancy rule.
+template <int G>
+static int launch_fixed_lag_vjp(dexr_robot* r, const dexr_params_t* prm, const dexr_fixed_lag_vjp_t* io, long long S, int K,
+                                cudaStream_t stream) {
+  FixedLagVjpArgs a{};
+  a.table = r->table_dev;
+  a.prm = *prm;
+  if (!(io->smooth_weight < 0.f)) a.prm.norm_delta = io->smooth_weight;
+  a.io = *io;
+  fixed_lag_vjp_layout(r->host, S, io->lag, io->workspace, &a.ws);
+  a.wio = fixed_lag_vjp_window_io(r->host, a.ws);
+  a.wpk = PackedLayout{a.ws.offsets, 2 * S, S * (io->lag + 1)};
+  a.S = S;
+  a.K = K;
+  a.dm = make_dims(r->host);
+  a.scratch_off = round_up((int)sizeof(SharedTable), 16);
+  constexpr int GPW = 32 / G;
+  a.pos_off = round_up(a.scratch_off + kEvalWarps * GPW * VjpScratch<G>::kFloats * 4, 16);
+  const int smem = a.pos_off + kEvalWarps * 2 * (int)sizeof(long long);
+  auto kern = dexr_fixed_lag_vjp_kernel<G>;
+  CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  int per_sm = 1;
+  if (int e = eval_ctas_per_sm(kern, smem, &per_sm)) return e;
+  const int grid = (int)std::min<long long>(S, (long long)r->num_sms * per_sm);
+  kern<<<grid, kEvalWarps * 32, smem, stream>>>(a);
+  CUDA_TRY(cudaGetLastError());
+  {
+    std::lock_guard<std::mutex> lk(r->info_mu);
+    r->last = dexr_launch_info_t{grid, kEvalWarps * 32, smem, 0, G, kEvalWarps, r->last.kernels_launched + 1};
+  }
+  return 0;
+}
+
+extern "C" size_t dexr_fixed_lag_vjp_sizeof(void) { return sizeof(dexr_fixed_lag_vjp_t); }
+
+extern "C" size_t dexr_fixed_lag_vjp_workspace_bytes(const dexr_robot_t* robot, int64_t num_streams, int32_t lag) {
+  return robot ? fixed_lag_vjp_workspace_bytes(robot->host, num_streams, lag) : 0;
+}
+
+extern "C" int dexr_fixed_lag_step_vjp(const dexr_robot_t* robot, const dexr_params_t* params, const dexr_fixed_lag_vjp_t* io,
+                                       int64_t num_streams, int64_t num_ticks, void* cuda_stream) {
+  if (!robot || !params || !io) return fail(DEXR_E_INVALID, "dexr_fixed_lag_step_vjp: null argument");
+  if (const char* msg = fixed_lag_vjp_io_error(robot->host, *io, *params, num_streams, num_ticks))
+    return fail(DEXR_E_INVALID, "%s", msg);
+  if (int e = check_loss_params(params)) return e;
+  if (num_streams == 0) return 0;
+  DEVICE_SCOPE(robot->device);
+  dexr_robot* r = const_cast<dexr_robot*>(robot);
+  cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
+  return eval_lanes(r->host) == 16 ? launch_fixed_lag_vjp<16>(r, params, io, num_streams, (int)num_ticks, stream)
+                                   : launch_fixed_lag_vjp<32>(r, params, io, num_streams, (int)num_ticks, stream);
 }
 
 extern "C" {

@@ -3261,11 +3261,14 @@ __device__ __forceinline__ float fixed_lag_emit(Solver<G, 0>& sv, const dexr_fix
 // read back after it for the same reason.  `owner`: this group runs the stream (the kernel gives a 16-lane warp's second
 // group none: it walks the same ticks with every read and write off, so that the warp's shuffles stay converged; it reads
 // window_len too).  `wstatus`: the status words after the smoother's part of the workspace.  Between a lane's global
-// writes and another lane's reads, __syncwarp.
-template <int G>
+// writes and another lane's reads, __syncwarp.  REC (dexr_fixed_lag_step_tape): after the solve, the window minimiser goes
+// to tape_qpos [S,K,L+1,n_var] and the committed flags the solve started from to tape_projected [S,K,len_proj] (nullptr:
+// none).
+template <int G, bool REC = false>
 __device__ __forceinline__ void fixed_lag_tick(Solver<G, 0>& sv, const dexr_fixed_lag_t& io, const Dims& dm,
                                                const dexr_params_t& prm, int32_t* wstatus, int K,
-                                               const volatile long long* pos, bool owner) {
+                                               const volatile long long* pos, bool owner, float* tape_qpos = nullptr,
+                                               uint8_t* tape_projected = nullptr) {
   constexpr int KP = 3 * DEXR_NUM_KEYPOINTS;
   const int l = sv.l, n = dm.n_var, nf = dm.n_fixed, L = io.lag, W1 = L + 1;
   const bool isvar = sv.var >= 0;
@@ -3296,6 +3299,13 @@ __device__ __forceinline__ void fixed_lag_tick(Solver<G, 0>& sv, const dexr_fixe
     sio.status_out = wstatus;
     sio.workspace = io.workspace;
     smooth_packed_stream(sv, sio, dm, prm, PackedStream{s, s * W1, io.window_len[s]}, owner, static_cast<float*>(io.workspace));
+  }
+  if constexpr (REC) {  // (each var lane copies the entries it wrote itself)
+    const long long s = pos[0], t = s * K + pos[1];
+    const int m = static_cast<const volatile int32_t*>(io.window_len)[s];
+    if (owner && isvar)
+      for (int j = 0; j < m; ++j) tape_qpos[(t * W1 + j) * n + sv.var] = io.window_qpos[(s * W1 + j) * n + sv.var];
+    if (owner && tape_projected && l < dm.len_proj) tape_projected[t * dm.len_proj + l] = io.projected[s * dm.len_proj + l];
   }
   // 3. emit slot 0 and commit it, or emit nothing
   const long long s = pos[0], fin = s * K + pos[1], w0 = s * W1;
@@ -3340,6 +3350,325 @@ __device__ __forceinline__ void fixed_lag_flush(Solver<G, 0>& sv, const dexr_fix
   if (owner && l == 0) {
     io.flush_count_out[s] = h;
     io.window_len[s] = 0;
+  }
+  __syncwarp();
+}
+
+// ------------------------------------------------------------------------------------------------
+// backpropagation through fixed-lag smoothing (dexr_fixed_lag_step_vjp, see dexr.h for the math): each differentiated tick's
+// window is rebuilt in the workspace as a one-stream packed clip and smooth_vjp_packed_stream runs unchanged on it
+// ------------------------------------------------------------------------------------------------
+// The workspace of a call on S streams of lag L, W1 = L + 1 frames per stream: the rebuilt windows (frames s W1 .. s W1 +
+// m - 1 of stream s) and their outputs, and the per-stream rows of the smoother's view.  Stream s is packed stream 2 s of
+// that view (offsets[2s], offsets[2s+1] bound its window), so that every window's range is its own two words; the odd
+// streams are never run.  Each array starts on a 16-byte boundary.
+struct FixedLagVjpWs {
+  int64_t* offsets;  // [2S]
+  float* smooth;     // [S W1] SmoothWs<G>::kFloats each: the smoother VJP's Z_t, y_t, v_t
+  float* kp;         // [S W1,21,3] the window's keypoints
+  float* fixed;      // [S W1,n_fixed]
+  float* qpos;       // [S W1,n_var] the point X^k
+  float* gq;         // [S W1,n_var] the window's qpos cotangent
+  float* grq;        // [S W1,dof] the window's robot_qpos cotangent
+  float* gkp;        // [S W1,21,3] the window VJP's keypoint cotangents
+  float* gfixed;     // [S W1,n_fixed]
+  int32_t* status;   // [S W1]
+  float* anchor;     // [2S,n_var] row 2s: A_k
+  float* ganchor;    // [2S,n_var] row 2s: the window VJP's anchor cotangent
+  float* abar;       // [S,n_var] the carried anchor cotangent
+  uint8_t* flags;    // [2S,len_proj] row 2s: the flags W_k's solve started from
+};
+
+// Lays the workspace of S streams of lag L out from `base` (may be nullptr) into `w`; returns its size in bytes.
+inline size_t fixed_lag_vjp_layout(const dexr_table_t& t, long long S, long long lag, void* base, FixedLagVjpWs* w) {
+  if (S <= 0 || lag < 0 || lag > DEXR_FIXED_LAG_MAX) return 0;
+  const long long F = S * (lag + 1);
+  const int floats = eval_lanes(t) == 16 ? SmoothWs<16>::kFloats : SmoothWs<32>::kFloats;
+  char* const b = static_cast<char*>(base);
+  size_t off = 0;
+  auto take = [&](size_t bytes) {
+    char* p = b ? b + off : nullptr;
+    off += (bytes + 15) & ~(size_t)15;
+    return static_cast<void*>(p);
+  };
+  FixedLagVjpWs r;
+  r.offsets = static_cast<int64_t*>(take((size_t)(2 * S) * sizeof(int64_t)));
+  r.smooth = static_cast<float*>(take((size_t)F * floats * sizeof(float)));
+  r.kp = static_cast<float*>(take((size_t)F * 3 * DEXR_NUM_KEYPOINTS * sizeof(float)));
+  r.fixed = static_cast<float*>(take((size_t)F * t.n_fixed * sizeof(float)));
+  r.qpos = static_cast<float*>(take((size_t)F * t.n_var * sizeof(float)));
+  r.gq = static_cast<float*>(take((size_t)F * t.n_var * sizeof(float)));
+  r.grq = static_cast<float*>(take((size_t)F * t.dof * sizeof(float)));
+  r.gkp = static_cast<float*>(take((size_t)F * 3 * DEXR_NUM_KEYPOINTS * sizeof(float)));
+  r.gfixed = static_cast<float*>(take((size_t)F * t.n_fixed * sizeof(float)));
+  r.status = static_cast<int32_t*>(take((size_t)F * sizeof(int32_t)));
+  r.anchor = static_cast<float*>(take((size_t)(2 * S) * t.n_var * sizeof(float)));
+  r.ganchor = static_cast<float*>(take((size_t)(2 * S) * t.n_var * sizeof(float)));
+  r.abar = static_cast<float*>(take((size_t)S * t.n_var * sizeof(float)));
+  r.flags = static_cast<uint8_t*>(take((size_t)(2 * S) * t.len_proj));
+  if (w) *w = r;
+  return off;
+}
+
+// dexr_fixed_lag_vjp_workspace_bytes.
+inline size_t fixed_lag_vjp_workspace_bytes(const dexr_table_t& t, long long S, long long lag) {
+  return fixed_lag_vjp_layout(t, S, lag, nullptr, nullptr);
+}
+
+// The smoother VJP's view of a laid-out workspace: packed clips of the rebuilt windows.
+inline dexr_smooth_vjp_t fixed_lag_vjp_window_io(const dexr_table_t& t, const FixedLagVjpWs& w) {
+  dexr_smooth_vjp_t v{};
+  v.keypoints = w.kp;
+  v.fixed_qpos = t.n_fixed > 0 ? w.fixed : nullptr;
+  v.last_qpos = w.anchor;
+  v.projected = t.len_proj > 0 ? w.flags : nullptr;
+  v.qpos = w.qpos;
+  v.grad_qpos = w.gq;
+  v.grad_robot_qpos = w.grq;
+  v.smooth_weight = -1.f;  // (not read by the kernel: params.norm_delta holds w)
+  v.workspace = w.smooth;
+  v.grad_keypoints = w.gkp;
+  v.grad_fixed_qpos = t.n_fixed > 0 ? w.gfixed : nullptr;
+  v.grad_last_qpos = w.ganchor;
+  v.status_out = w.status;
+  return v;
+}
+
+// The argument checks of dexr_fixed_lag_step_tape's tape: nullptr, or what is wrong.
+inline const char* fixed_lag_tape_error(const dexr_table_t& t, const dexr_fixed_lag_tape_t* tape) {
+  if (!tape || !tape->qpos) return "tape->qpos is required";
+  if (t.len_proj > 0 && !tape->projected) return "DexPilot: the flag tape needs tape->projected";
+  return nullptr;
+}
+
+// The argument checks of dexr_fixed_lag_step_vjp: nullptr, or what is wrong.  Host code shared by the library and the host
+// emulation.
+inline const char* fixed_lag_vjp_io_error(const dexr_table_t& t, const dexr_fixed_lag_vjp_t& io, const dexr_params_t& prm,
+                                          long long S, long long K) {
+  if (S < 0 || K < 0 || K > INT32_MAX) return "bad sizes: num_streams and num_ticks must be >= 0, num_ticks <= INT32_MAX";
+  if (io.lag < 0 || io.lag > DEXR_FIXED_LAG_MAX) return "lag must be in 0..4095";
+  if (S > INT32_MAX / (2 * ((long long)io.lag + 1))) return "num_streams * (lag + 1) must be <= INT32_MAX / 2";
+  if (prm.preprocess != 0) return "raw landmarks are not differentiated: params.preprocess must be 0 (pre-process the keypoints first)";
+  if (!io.last_qpos || !io.window_len) return "last_qpos and window_len (the state before the call) are required";
+  if (K > 0 && (!io.keypoints || !io.window_keypoints || !io.tape.qpos || !io.grad_keypoints))
+    return "keypoints, window_keypoints, tape.qpos and grad_keypoints are required";
+  if (K > 0 && t.len_proj > 0 && !io.tape.projected) return "DexPilot: tape.projected is required";
+  if (K > 0 && t.n_fixed > 0 && (!io.fixed_qpos || !io.window_fixed_qpos))
+    return "the robot has fixed joints but fixed_qpos or window_fixed_qpos is NULL";
+  if (!(io.smooth_weight < 0.f) && !(io.smooth_weight >= 0.f && io.smooth_weight <= 3.0e38f))
+    return "smooth_weight must be finite (< 0: params.norm_delta)";
+  if (S > 0 && (!io.workspace || io.workspace_bytes < fixed_lag_vjp_workspace_bytes(t, S, io.lag)))
+    return "workspace smaller than dexr_fixed_lag_vjp_workspace_bytes(robot, num_streams, lag)";
+  return nullptr;
+}
+
+// Where a stream's call ends (group-uniform): h0 the held frames at the start, hend those held after the ticks (before a
+// flush), cend the frames committed by then (final slot i holds input frame cend + i), elast whether the last tick emitted
+// and `route` where grad_last_qpos_out goes: 0 the incoming anchor, 1 slot 0 of the last window, 2 its last held slot.
+struct FixedLagEnd {
+  int h0, hend, cend, elast, route;
+};
+__device__ __forceinline__ FixedLagEnd fixed_lag_end(int h0_raw, int L, int K, bool flushed) {
+  FixedLagEnd e;
+  e.h0 = h0_raw < 0 ? 0 : (h0_raw > L ? L : h0_raw);
+  const int mlast = K > 0 ? (e.h0 + K < L + 1 ? e.h0 + K : L + 1) : e.h0;
+  e.elast = (K > 0 && mlast == L + 1) ? 1 : 0;
+  e.hend = mlast - e.elast;
+  e.cend = e.h0 + K - L > 0 ? e.h0 + K - L : 0;
+  e.route = (flushed && e.hend > 0) ? 2 : (e.elast ? 1 : 0);
+  return e;
+}
+
+// smooth_vjp_packed_stream's cotangent of a var lane: M^T r (r: this lane's joint's robot_qpos cotangent, the mimic
+// followers folded into their source) + gq, in its order of operations, so that a cotangent folded here and one folded by
+// the window VJP give the same bits.
+template <int G>
+__device__ __forceinline__ float fixed_lag_fold(const Solver<G, 0>& sv, const Dims& dm, float r, float gq) {
+  const SharedTable& st = Solver<G, 0>::ST();
+  const int l = sv.l;
+  const bool isvar = sv.var >= 0;
+  float gb = r;
+  if (dm.has_mimic) {
+    const int gcount = st.group_count[l];
+    float gx_ = 0.f;
+#pragma unroll
+    for (int k = 0; k < DEXR_MAX_GROUP; ++k) {
+      const bool v = isvar && k < gcount;
+      const float gv = gshfl<G>(r, v ? st.group_lane[l][k] : l);
+      if (v) gx_ = fmaf(st.group_mult[l][k], gv, gx_);
+    }
+    gb = gx_;
+  }
+  gb += gq;
+  return isvar ? gb : 0.f;
+}
+
+// The start of stream s (< S) of dexr_fixed_lag_step_vjp: every output row of the stream written once (zeros, PENDING), the
+// final state's keypoint and fixed-joint cotangents onto the input frames their held slots hold (the flushed rows' fixed-joint
+// share too: those frames' sums start with it, so a chunked run gives the same bits; unlike the window VJP's direct term
+// it is kept on a NOT_PD window or a missing frame, see dexr.h), the anchor's own cotangent when it routes there, the carried abar zeroed.
+// With K = 0 the flush rows are the incoming held slots of window_qpos.  `owner` as in fixed_lag_tick.
+template <int G>
+__device__ __forceinline__ void fixed_lag_vjp_begin(const Solver<G, 0>& sv, const dexr_fixed_lag_vjp_t& io,
+                                                    const FixedLagVjpWs& ws, const Dims& dm, long long s, int K,
+                                                    bool owner) {
+  constexpr int KP = 3 * DEXR_NUM_KEYPOINTS;
+  const int l = sv.l, n = dm.n_var, nf = dm.n_fixed, dof = dm.dof, L = io.lag, W1 = L + 1;
+  const bool isvar = sv.var >= 0;
+  const int fixedi = Solver<G, 0>::ST().fixed_index[l];
+  const FixedLagEnd e = fixed_lag_end(io.window_len[s], L, K, io.flushed != 0);
+  if (owner) {
+    for (int k = 0; k < K; ++k) {
+      for (int c = l; c < KP; c += G) io.grad_keypoints[(s * K + k) * KP + c] = 0.f;
+      if (fixedi >= 0 && io.grad_fixed_qpos) io.grad_fixed_qpos[(s * K + k) * nf + fixedi] = 0.f;
+      if (l == 0 && io.status_out) io.status_out[s * K + k] = DEXR_STATUS_PENDING;
+    }
+    for (int j = 0; j < W1; ++j) {
+      if (io.grad_window_keypoints)
+        for (int c = l; c < KP; c += G) io.grad_window_keypoints[(s * W1 + j) * KP + c] = 0.f;
+      if (fixedi >= 0 && io.grad_window_fixed_qpos) io.grad_window_fixed_qpos[(s * W1 + j) * nf + fixedi] = 0.f;
+      if (isvar && io.grad_window_qpos) io.grad_window_qpos[(s * W1 + j) * n + sv.var] = 0.f;
+    }
+    if (isvar) {
+      if (io.grad_last_qpos)
+        io.grad_last_qpos[s * n + sv.var] = (e.route == 0 && io.grad_last_qpos_out) ? io.grad_last_qpos_out[s * n + sv.var] : 0.f;
+      ws.abar[s * n + sv.var] = 0.f;
+    }
+    // the final state's held slots: slot i holds input frame g = cend + i (held at the start when g < h0)
+    for (int i = 0; i < e.hend; ++i) {
+      const int g = e.cend + i;
+      const bool held = g < e.h0;
+      if (io.grad_window_keypoints_out) {
+        float* const d = held ? io.grad_window_keypoints : io.grad_keypoints;
+        const long long row = held ? s * W1 + g : s * K + (g - e.h0);
+        if (d)
+          for (int c = l; c < KP; c += G) d[row * KP + c] = io.grad_window_keypoints_out[(s * W1 + i) * KP + c];
+      }
+      if (fixedi >= 0) {
+        float* const d = held ? io.grad_window_fixed_qpos : io.grad_fixed_qpos;
+        const long long row = held ? s * W1 + g : s * K + (g - e.h0);
+        float v = io.grad_window_fixed_qpos_out ? io.grad_window_fixed_qpos_out[(s * W1 + i) * nf + fixedi] : 0.f;
+        if (io.flushed && io.grad_flush_robot_qpos) v += io.grad_flush_robot_qpos[(s * L + i) * dof + l];
+        if (d) d[row * nf + fixedi] = v;
+      }
+    }
+  }
+  __syncwarp();
+  if (K == 0) {  // (uniform) the held slots of window_qpos are the flushed rows and the final window_qpos
+    for (int j = 0; j < e.h0; ++j) {
+      const float r = (owner && l < dof && io.flushed && io.grad_flush_robot_qpos && fixedi < 0)
+                          ? io.grad_flush_robot_qpos[(s * L + j) * dof + l] : 0.f;
+      float q = 0.f;
+      if (owner && isvar) {
+        q = io.grad_window_qpos_out ? io.grad_window_qpos_out[(s * W1 + j) * n + sv.var] : 0.f;
+        q += (io.flushed && io.grad_flush_qpos) ? io.grad_flush_qpos[(s * L + j) * n + sv.var] : 0.f;
+        if (e.route == 2 && j == e.h0 - 1 && io.grad_last_qpos_out) q += io.grad_last_qpos_out[s * n + sv.var];
+      }
+      const float gb = fixed_lag_fold(sv, dm, r, q);
+      if (owner && isvar && io.grad_window_qpos) io.grad_window_qpos[(s * W1 + j) * n + sv.var] = gb;
+    }
+  }
+  __syncwarp();
+}
+
+// Rebuilds the window of tick pos[1] of stream pos[0] of dexr_fixed_lag_step_vjp in the workspace (frames, fixed joints,
+// point, anchor, flags and the slot cotangents, see dexr.h) when the tick is differentiated -- it emits or is the last --
+// and returns whether it is (group-uniform).  `owner` as in fixed_lag_tick.
+template <int G>
+__device__ __forceinline__ bool fixed_lag_vjp_rebuild(const Solver<G, 0>& sv, const dexr_fixed_lag_vjp_t& io,
+                                                      const FixedLagVjpWs& ws, const Dims& dm, int K,
+                                                      const volatile long long* pos, bool owner) {
+  constexpr int KP = 3 * DEXR_NUM_KEYPOINTS;
+  const int l = sv.l, n = dm.n_var, nf = dm.n_fixed, dof = dm.dof, L = io.lag, W1 = L + 1;
+  const long long s = pos[0];
+  const int k = (int)pos[1];
+  const FixedLagEnd e = fixed_lag_end(io.window_len[s], L, K, io.flushed != 0);
+  const int m = e.h0 + k + 1 < W1 ? e.h0 + k + 1 : W1, c0 = e.h0 + k - L > 0 ? e.h0 + k - L : 0;
+  const bool emit = m == W1, last = k == K - 1;
+  if (!emit && !last) {
+    __syncwarp();  // (every lane has read the loop state and window_len before lane 0 advances the loop)
+    return false;
+  }
+  const bool isvar = sv.var >= 0;
+  const int fixedi = Solver<G, 0>::ST().fixed_index[l];
+  const long long t = s * K + k, w0 = s * W1;
+  if (owner) {
+    for (int j = 0; j < m; ++j) {
+      const int g = c0 + j;
+      const bool held = g < e.h0;
+      const long long src = held ? s * W1 + g : s * K + (g - e.h0);
+      const float* const kp = held ? io.window_keypoints : io.keypoints;
+      for (int c = l; c < KP; c += G) ws.kp[(w0 + j) * KP + c] = kp[src * KP + c];
+      if (fixedi >= 0) ws.fixed[(w0 + j) * nf + fixedi] = (held ? io.window_fixed_qpos : io.fixed_qpos)[src * nf + fixedi];
+      // the slot's cotangents: slot 0 of an emitting tick its emitted row (+ abar, or grad_last_qpos_out on the last tick);
+      // on the last tick the slots still held after it (final slot i = j - elast) the final state's and the flush's
+      const int i = j - e.elast;
+      const bool row = emit && j == 0, tail = last && i >= 0;
+      if (isvar) {
+        ws.qpos[(w0 + j) * n + sv.var] = io.tape.qpos[(t * W1 + j) * n + sv.var];
+        float q = 0.f;
+        if (row) {
+          q = io.grad_qpos ? io.grad_qpos[t * n + sv.var] : 0.f;
+          if (!last) q += ws.abar[s * n + sv.var];
+          else if (e.route == 1 && io.grad_last_qpos_out) q += io.grad_last_qpos_out[s * n + sv.var];
+        } else if (tail) {
+          q = io.grad_window_qpos_out ? io.grad_window_qpos_out[(w0 + i) * n + sv.var] : 0.f;
+          q += (io.flushed && io.grad_flush_qpos) ? io.grad_flush_qpos[(s * L + i) * n + sv.var] : 0.f;
+          if (e.route == 2 && i == e.hend - 1 && io.grad_last_qpos_out) q += io.grad_last_qpos_out[s * n + sv.var];
+        }
+        ws.gq[(w0 + j) * n + sv.var] = q;
+      }
+      if (l < dof) {  // (a flushed row's fixed-joint share went to the frame's sum in fixed_lag_vjp_begin)
+        float r = 0.f;
+        if (row) r = io.grad_robot_qpos ? io.grad_robot_qpos[t * dof + l] : 0.f;
+        else if (tail && fixedi < 0 && io.flushed && io.grad_flush_robot_qpos) r = io.grad_flush_robot_qpos[(s * L + i) * dof + l];
+        ws.grq[(w0 + j) * dof + l] = r;
+      }
+    }
+    if (isvar) ws.anchor[2 * s * n + sv.var] = c0 == 0 ? io.last_qpos[s * n + sv.var] : io.tape.qpos[((t - 1) * W1) * n + sv.var];
+    if (l < dm.len_proj) ws.flags[2 * s * dm.len_proj + l] = io.tape.projected[t * dm.len_proj + l];
+    if (l == 0) {
+      ws.offsets[2 * s] = w0;
+      ws.offsets[2 * s + 1] = w0 + m;
+    }
+  }
+  __syncwarp();
+  return true;
+}
+
+// After the window VJP of tick pos[1] of stream pos[0]: its frames' cotangents added to the input frames they came from, its
+// anchor cotangent carried to the previous tick's slot 0 (c_k >= 1) or added to grad_last_qpos (c_k = 0), the emitted
+// frame's status.
+template <int G>
+__device__ __forceinline__ void fixed_lag_vjp_scatter(const Solver<G, 0>& sv, const dexr_fixed_lag_vjp_t& io,
+                                                      const FixedLagVjpWs& ws, const Dims& dm, int K,
+                                                      const volatile long long* pos, bool owner) {
+  constexpr int KP = 3 * DEXR_NUM_KEYPOINTS;
+  const int l = sv.l, n = dm.n_var, nf = dm.n_fixed, L = io.lag, W1 = L + 1;
+  const long long s = pos[0];
+  const int k = (int)pos[1];
+  const int h0r = io.window_len[s];
+  const int h0 = h0r < 0 ? 0 : (h0r > L ? L : h0r);
+  const int m = h0 + k + 1 < W1 ? h0 + k + 1 : W1, c0 = h0 + k - L > 0 ? h0 + k - L : 0;
+  const int fixedi = Solver<G, 0>::ST().fixed_index[l];
+  const long long w0 = s * W1;
+  if (owner) {
+    for (int j = 0; j < m; ++j) {
+      const int g = c0 + j;
+      const bool held = g < h0;
+      const long long row = held ? s * W1 + g : s * K + (g - h0);
+      float* const d = held ? io.grad_window_keypoints : io.grad_keypoints;
+      if (d)
+        for (int c = l; c < KP; c += G) d[row * KP + c] += ws.gkp[(w0 + j) * KP + c];
+      float* const df = held ? io.grad_window_fixed_qpos : io.grad_fixed_qpos;
+      if (fixedi >= 0 && df) df[row * nf + fixedi] += ws.gfixed[(w0 + j) * nf + fixedi];
+    }
+    if (sv.var >= 0) {
+      const float ab = ws.ganchor[2 * s * n + sv.var];
+      if (c0 > 0) ws.abar[s * n + sv.var] = ab;
+      else if (io.grad_last_qpos) io.grad_last_qpos[s * n + sv.var] += ab;
+    }
+    if (l == 0 && io.status_out && m == W1) io.status_out[s * K + k] = ws.status[w0];
   }
   __syncwarp();
 }

@@ -259,3 +259,98 @@ def differentiable_smooth_packed_sequences(seq, keypoints, layout, state=None, f
         smooth_weight = float(smooth_weight)
     cfg = dict(state=state, layout=layout, qpos_init=qpos_init, smooth_weight=smooth_weight)
     return _DifferentiableSmoothPackedSequences.apply(keypoints, fixed_qpos, state.last_qpos, seq, cfg)
+
+
+def _fixed_lag_copy(state):
+    """A detached copy of a FixedLagState (the forward updates its state in place; autograd keeps the original)."""
+    from .seq_retarget import FixedLagState
+
+    return FixedLagState(lag=state.lag, **{k: (None if getattr(state, k) is None else getattr(state, k).detach().clone())
+                                           for k in FixedLagState._FIELDS})
+
+
+class _DifferentiableRetargetFixedLag(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, keypoints, fixed_qpos, last_qpos, window_keypoints, window_fixed_qpos, window_qpos, seq, cfg):
+        state0 = _fixed_lag_copy(cfg["state"])
+        new = _fixed_lag_copy(state0)
+        S, K = int(keypoints.shape[0]), int(keypoints.shape[1])
+        tape = seq.make_fixed_lag_tape(S, K, state0.lag)
+        kp = keypoints.detach().contiguous()
+        fixed = None if fixed_qpos is None else fixed_qpos.detach().contiguous()
+        rq, q, status = seq.retarget_fixed_lag(kp, new, fixed_qpos=fixed, smooth_weight=cfg["smooth_weight"], tape=tape)
+        ctx.seq, ctx.tape, ctx.state0, ctx.smooth_weight = seq, tape, state0, cfg["smooth_weight"]
+        ctx.save_for_backward(kp, fixed)
+        ctx.set_materialize_grads(False)
+        ctx.mark_non_differentiable(status)
+        cfg["new_state"] = new
+        return rq, q, status, new.last_qpos, new.window_keypoints, new.window_fixed_qpos, new.window_qpos
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g_rq, g_q, _g_status, g_last, g_wkp, g_wfix, g_wq):
+        kp, fixed = ctx.saved_tensors
+        c = (lambda g: None if g is None else g.contiguous())
+        g_kp, g_fixed, g_last0, g_wkp0, g_wfix0, g_wq0, _ = ctx.seq.retarget_fixed_lag_vjp(
+            kp, ctx.tape, ctx.state0, fixed_qpos=fixed, grad_qpos=c(g_q), grad_robot_qpos=c(g_rq),
+            grad_last_qpos_out=c(g_last), grad_window_qpos_out=c(g_wq), grad_window_keypoints_out=c(g_wkp),
+            grad_window_fixed_qpos_out=c(g_wfix), smooth_weight=ctx.smooth_weight)
+        return g_kp, g_fixed, g_last0, g_wkp0, g_wfix0, g_wq0, None, None
+
+
+def differentiable_retarget_fixed_lag(seq, keypoints, state, fixed_qpos=None, *, smooth_weight=None):
+    """(robot_qpos [S,K,dof], qpos [S,K,opt_dof], status [S,K], new_state) = `seq.retarget_fixed_lag(keypoints, state,
+    ...)` (float32 CUDA tensors as there), differentiable in `keypoints`, `fixed_qpos` and the state's `last_qpos`,
+    `window_keypoints`, `window_fixed_qpos` and `window_qpos`.  The contract of `differentiable_retarget_sequences`: `state`
+    is not modified, and the returned FixedLagState's last_qpos and window tensors carry the graph, so chunks of a live
+    stream backpropagate across call boundaries (detach the state for truncated backpropagation).  backward() is one
+    `retarget_fixed_lag_vjp` launch: each emitting window's smoother VJP, the anchor chain through the committed frames.
+    PENDING rows (NaN) get no gradient.  The DexPilot flags and `smooth_weight` are not differentiated."""
+    from .seq_retarget import FixedLagState
+
+    if isinstance(smooth_weight, torch.Tensor):
+        if smooth_weight.requires_grad:
+            raise ValueError("smooth_weight requires grad, but fixed-lag smoothing is not differentiated in it: detach it")
+        smooth_weight = float(smooth_weight)
+    cfg = dict(state=state, smooth_weight=smooth_weight)
+    rq, q, status, last, wkp, wfix, wq = _DifferentiableRetargetFixedLag.apply(
+        keypoints, fixed_qpos, state.last_qpos, state.window_keypoints, state.window_fixed_qpos, state.window_qpos, seq, cfg)
+    new = cfg["new_state"]
+    return rq, q, status, FixedLagState(lag=new.lag, last_qpos=last, projected=new.projected, window_keypoints=wkp,
+                                        window_fixed_qpos=wfix, window_qpos=wq, window_len=new.window_len)
+
+
+class _DifferentiableFlushFixedLag(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, last_qpos, window_keypoints, window_fixed_qpos, window_qpos, seq, cfg):
+        state0 = _fixed_lag_copy(cfg["state"])
+        new = _fixed_lag_copy(state0)
+        rq, q, count = seq.flush_fixed_lag(new)
+        ctx.seq, ctx.state0 = seq, state0
+        ctx.set_materialize_grads(False)
+        ctx.mark_non_differentiable(count)
+        cfg["new_state"] = new
+        return rq, q, count, new.last_qpos, new.window_keypoints, new.window_fixed_qpos, new.window_qpos
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g_rq, g_q, _g_count, g_last, g_wkp, g_wfix, g_wq):
+        c = (lambda g: None if g is None else g.contiguous())
+        g_last0, g_wkp0, g_wfix0, g_wq0 = ctx.seq.flush_fixed_lag_vjp(
+            ctx.state0, grad_qpos=c(g_q), grad_robot_qpos=c(g_rq), grad_last_qpos_out=c(g_last),
+            grad_window_qpos_out=c(g_wq), grad_window_keypoints_out=c(g_wkp), grad_window_fixed_qpos_out=c(g_wfix))
+        return g_last0, g_wkp0, g_wfix0, g_wq0, None, None
+
+
+def differentiable_flush_fixed_lag(seq, state):
+    """(robot_qpos [S,L,dof], qpos [S,L,opt_dof], count [S], new_state) = `seq.flush_fixed_lag(state)`, differentiable in
+    the state's `last_qpos` and window tensors (the flushed rows are its held slots of window_qpos).  `state` is not
+    modified; the returned state carries the graph as `differentiable_retarget_fixed_lag`'s does."""
+    from .seq_retarget import FixedLagState
+
+    cfg = dict(state=state)
+    rq, q, count, last, wkp, wfix, wq = _DifferentiableFlushFixedLag.apply(
+        state.last_qpos, state.window_keypoints, state.window_fixed_qpos, state.window_qpos, seq, cfg)
+    new = cfg["new_state"]
+    return rq, q, count, FixedLagState(lag=new.lag, last_qpos=last, projected=new.projected, window_keypoints=wkp,
+                                       window_fixed_qpos=wfix, window_qpos=wq, window_len=new.window_len)

@@ -122,6 +122,15 @@ class FixedLagState:
 
 
 @dataclass
+class FixedLagTape:
+    """What a recorded `retarget_fixed_lag` call leaves for its backward (`dexr_fixed_lag_tape_t`): torch tensors on the
+    optimizer's device.  S K (L+1) opt_dof floats: 84 MB at S = 256, K = 300, L = 16, opt_dof = 16."""
+
+    qpos: "torch.Tensor"                 # [S, K, L+1, opt_dof] float32: each tick's window minimiser
+    projected: Optional["torch.Tensor"]  # [S, K, len_proj] uint8: the committed flags each tick's solve started from, or None
+
+
+@dataclass
 class SequenceTape:
     """What a recorded `retarget_sequences` call leaves for its backward (`dexr_sequences_tape_t`): torch tensors on the
     optimizer's device."""
@@ -778,8 +787,22 @@ class SeqRetargeting:
             window_qpos=torch.zeros((num_streams, lag + 1, opt.opt_dof), dtype=torch.float32, device=dev),
             window_len=torch.zeros((num_streams,), dtype=torch.int32, device=dev))
 
-    def _fixed_lag_call(self, state: FixedLagState, K: int, fill, smooth_weight, stream):
-        """One `dexr_fixed_lag_step` call on `state` with K ticks; `fill(io, chk)` sets the per-call buffers."""
+    def make_fixed_lag_tape(self, num_streams: int, num_ticks: int, lag: int) -> FixedLagTape:
+        """Buffers for recording a `retarget_fixed_lag` call of K ticks on S streams of lag L (`tape=`), the input of
+        `retarget_fixed_lag_vjp`."""
+        import torch
+
+        opt = self.optimizer
+        dev = torch.device("cuda", opt.engine().device)
+        len_proj = opt._objective_spec().len_proj
+        S, K, L = int(num_streams), int(num_ticks), int(lag)
+        return FixedLagTape(
+            qpos=torch.empty((S, K, L + 1, opt.opt_dof), dtype=torch.float32, device=dev),
+            projected=torch.empty((S, K, len_proj), dtype=torch.uint8, device=dev) if len_proj else None)
+
+    def _fixed_lag_call(self, state: FixedLagState, K: int, fill, smooth_weight, stream, tape: Optional[FixedLagTape] = None):
+        """One `dexr_fixed_lag_step` call on `state` with K ticks (`dexr_fixed_lag_step_tape` into `tape` when given);
+        `fill(io, chk)` sets the per-call buffers."""
         import torch
 
         opt = self.optimizer
@@ -811,12 +834,22 @@ class SeqRetargeting:
         io.workspace, io.workspace_bytes = ws.data_ptr(), nbytes
         s = stream if stream is not None else torch.cuda.current_stream(dev)
         p = opt.params(clip_init=True, lp_alpha=self.low_pass_alpha)
-        N.check(eng.lib.dexr_fixed_lag_step(eng.handle, C.byref(p), C.byref(io), S, K, C.c_void_p(s.cuda_stream)),
-                "dexr_fixed_lag_step")
+        if tape is None:
+            N.check(eng.lib.dexr_fixed_lag_step(eng.handle, C.byref(p), C.byref(io), S, K, C.c_void_p(s.cuda_stream)),
+                    "dexr_fixed_lag_step")
+        else:
+            tp = N.DexrFixedLagTape()
+            tp.qpos = chk(tape.qpos, (S, K, L + 1, n), torch.float32, "tape.qpos")
+            if len_proj:
+                if tape.projected is None:
+                    raise ValueError("DexPilot streams need tape.projected")
+                tp.projected = chk(tape.projected, (S, K, len_proj), torch.uint8, "tape.projected")
+            N.check(eng.lib.dexr_fixed_lag_step_tape(eng.handle, C.byref(p), C.byref(io), C.byref(tp), S, K,
+                                                     C.c_void_p(s.cuda_stream)), "dexr_fixed_lag_step_tape")
         ws.record_stream(s)
 
     def retarget_fixed_lag(self, keypoints, state: FixedLagState, *, fixed_qpos=None, smooth_weight=None, out=None,
-                           qpos_out=None, status_out=None, stream=None):
+                           qpos_out=None, status_out=None, stream=None, tape: Optional[FixedLagTape] = None):
         """Fixed-lag smoothing of S live streams (`dexr_fixed_lag_step`, one launch): each of the K new frames per stream
         (keypoints [S,K,21,3], wrist-centred; fixed_qpos [S,K,n_fixed]) re-solves the last L+1 frames of its stream jointly
         with the offline smoother (`smooth_packed_sequences`, anchored at the last committed frame, w = smooth_weight or
@@ -824,7 +857,8 @@ class SeqRetargeting:
         STATUS_PENDING.  L = 0 is the causal problem; a dropped detection (NaN keypoints) is interpolated from both sides
         (STATUS_MISSING).  `state` (`make_fixed_lag_state`) is updated in place.  Returns (robot_qpos [S,K,dof] (scatter +
         mimic, no low-pass filter), qpos [S,K,opt_dof], status [S,K] int32), into `out` / `qpos_out` / `status_out` when
-        given.  Allocates its workspace on the device; nothing is synchronised."""
+        given.  `tape` (`make_fixed_lag_tape(S, K, L)`): also record what `retarget_fixed_lag_vjp` needs; the outputs and
+        the state are the same bits either way.  Allocates its workspace on the device; nothing is synchronised."""
         import torch
 
         opt = self.optimizer
@@ -849,7 +883,7 @@ class SeqRetargeting:
             io.robot_qpos_out = chk(out, (S, K, dof), torch.float32, "out")
             io.status_out = chk(status_out, (S, K), torch.int32, "status_out")
 
-        self._fixed_lag_call(state, K, fill, smooth_weight, stream)
+        self._fixed_lag_call(state, K, fill, smooth_weight, stream, tape)
         return out, qpos, status_out
 
     def flush_fixed_lag(self, state: FixedLagState, *, out=None, qpos_out=None, count_out=None, stream=None):
@@ -873,3 +907,138 @@ class SeqRetargeting:
 
         self._fixed_lag_call(state, 0, fill, None, stream)
         return rq, qpos, count
+
+    def _fixed_lag_vjp_call(self, state0: FixedLagState, K: int, fill, flushed: bool, smooth_weight, grads: dict, stream,
+                            outputs: Optional[dict] = None):
+        """One `dexr_fixed_lag_step_vjp` call: `state0` the state before the forward, `fill(io, chk, new)` the per-call
+        buffers, `grads` the final state's cotangents (None = 0), `outputs` tensors to write the outputs into, by their
+        dexr_fixed_lag_vjp_t names (the others are allocated).  Returns (grad_last_qpos, grad_window_keypoints,
+        grad_window_fixed_qpos or None, grad_window_qpos) of state0."""
+        import torch
+
+        opt = self.optimizer
+        eng = opt.engine()
+        dev = torch.device("cuda", eng.device)
+        chk = _checker(dev)
+        S, L = int(state0.last_qpos.shape[0]), int(state0.lag)
+        n, nf = opt.opt_dof, len(opt.idx_pin2fixed)
+        io = N.DexrFixedLagVjp()
+        io.lag, io.flushed = L, int(bool(flushed))
+        io.smooth_weight = -1.0 if smooth_weight is None else float(smooth_weight)
+        io.last_qpos = chk(state0.last_qpos, (S, n), torch.float32, "state0.last_qpos")
+        io.window_keypoints = chk(state0.window_keypoints, (S, L + 1, N.NUM_KEYPOINTS, 3), torch.float32,
+                                  "state0.window_keypoints")
+        if nf:
+            if state0.window_fixed_qpos is None:
+                raise ValueError(f"Optimizer has {nf} fixed joints but state0.window_fixed_qpos is None")
+            io.window_fixed_qpos = chk(state0.window_fixed_qpos, (S, L + 1, nf), torch.float32, "state0.window_fixed_qpos")
+        io.window_len = chk(state0.window_len, (S,), torch.int32, "state0.window_len")
+        shapes = dict(grad_last_qpos_out=(S, n), grad_window_qpos_out=(S, L + 1, n),
+                      grad_window_keypoints_out=(S, L + 1, N.NUM_KEYPOINTS, 3), grad_window_fixed_qpos_out=(S, L + 1, nf))
+        for k, shape in shapes.items():
+            g = grads.get(k)
+            if g is not None and (nf or k != "grad_window_fixed_qpos_out"):
+                setattr(io, k, chk(g, shape, torch.float32, k))
+
+        outputs = outputs or {}
+        unknown = set(outputs) - {"grad_keypoints", "grad_fixed_qpos", "grad_last_qpos", "grad_window_keypoints",
+                                  "grad_window_fixed_qpos", "grad_window_qpos", "status_out"}
+        if unknown:
+            raise ValueError(f"outputs: unknown names {sorted(unknown)}")
+
+        def new(shape, name, dtype=torch.float32):
+            t = outputs.get(name)
+            if t is None:
+                t = torch.empty(shape, dtype=dtype, device=dev)
+            setattr(io, name, chk(t, shape, dtype, f"outputs[{name!r}]"))
+            return t
+
+        g_last = new((S, n), "grad_last_qpos")
+        g_wkp = new((S, L + 1, N.NUM_KEYPOINTS, 3), "grad_window_keypoints")
+        g_wfix = new((S, L + 1, nf), "grad_window_fixed_qpos") if nf else None
+        g_wq = new((S, L + 1, n), "grad_window_qpos")
+        fill(io, chk, new)
+        nbytes = int(eng.lib.dexr_fixed_lag_vjp_workspace_bytes(eng.handle, S, L))
+        ws = torch.empty((max(nbytes, 4),), dtype=torch.uint8, device=dev)
+        io.workspace, io.workspace_bytes = ws.data_ptr(), nbytes
+        s = stream if stream is not None else torch.cuda.current_stream(dev)
+        p = opt.params(clip_init=True, lp_alpha=self.low_pass_alpha)
+        N.check(eng.lib.dexr_fixed_lag_step_vjp(eng.handle, C.byref(p), C.byref(io), S, K, C.c_void_p(s.cuda_stream)),
+                "dexr_fixed_lag_step_vjp")
+        ws.record_stream(s)
+        return g_last, g_wkp, g_wfix, g_wq
+
+    def retarget_fixed_lag_vjp(self, keypoints, tape: FixedLagTape, state0: FixedLagState, *, fixed_qpos=None,
+                               grad_qpos=None, grad_robot_qpos=None, grad_last_qpos_out=None, grad_window_qpos_out=None,
+                               grad_window_keypoints_out=None, grad_window_fixed_qpos_out=None, smooth_weight=None,
+                               stream=None, outputs: Optional[dict] = None):
+        """Backpropagation through a recorded `retarget_fixed_lag` call (`dexr_fixed_lag_step_vjp`, one launch): the
+        reverse-time VJP of its emitted rows (grad_qpos [S,K,opt_dof], grad_robot_qpos [S,K,dof]) and of the state it left
+        (grad_last_qpos_out [S,opt_dof], grad_window_*_out [S,L+1,...]) with respect to its frames and `state0`, the state
+        before the call (a copy: the forward updates its state in place).  Each emitting tick's window, and the last
+        tick's, is differentiated as `smooth_packed_sequences_vjp` differentiates a clip, at the minimiser the tape holds;
+        the anchor cotangent runs back through the committed frames.  Cotangents on PENDING rows are ignored.  Returns
+        (grad_keypoints [S,K,21,3], grad_fixed_qpos [S,K,n_fixed] or None, grad_last_qpos [S,opt_dof],
+        grad_window_keypoints [S,L+1,21,3], grad_window_fixed_qpos [S,L+1,n_fixed] or None, grad_window_qpos [S,L+1,opt_dof]
+        (zero: a warm start), status [S,K] int32 (the emitted frame's window status, STATUS_PENDING elsewhere)).
+        Chunks chained through these state cotangents give the same bits as one call.  `outputs`: tensors to write into,
+        by their dexr_fixed_lag_vjp_t names (grad_keypoints, ..., status_out).  Nothing is synchronised."""
+        import torch
+
+        opt = self.optimizer
+        if keypoints.dim() != 4 or tuple(keypoints.shape[2:]) != (N.NUM_KEYPOINTS, 3):
+            raise ValueError(f"keypoints must have shape [S,K,21,3], got {tuple(keypoints.shape)}")
+        S, K, L = int(keypoints.shape[0]), int(keypoints.shape[1]), int(state0.lag)
+        n, dof, nf = opt.opt_dof, opt.robot.dof, len(opt.idx_pin2fixed)
+        len_proj = opt._objective_spec().len_proj
+        res = {}
+
+        def fill(io, chk, new):
+            io.keypoints = chk(keypoints, (S, K, N.NUM_KEYPOINTS, 3), torch.float32, "keypoints")
+            if nf:
+                if fixed_qpos is None:
+                    raise ValueError(f"Optimizer has {nf} fixed joints but no fixed_qpos is given")
+                io.fixed_qpos = chk(fixed_qpos, (S, K, nf), torch.float32, "fixed_qpos")
+            io.tape.qpos = chk(tape.qpos, (S, K, L + 1, n), torch.float32, "tape.qpos")
+            if len_proj:
+                if tape.projected is None:
+                    raise ValueError("DexPilot streams need tape.projected")
+                io.tape.projected = chk(tape.projected, (S, K, len_proj), torch.uint8, "tape.projected")
+            if grad_qpos is not None:
+                io.grad_qpos = chk(grad_qpos, (S, K, n), torch.float32, "grad_qpos")
+            if grad_robot_qpos is not None:
+                io.grad_robot_qpos = chk(grad_robot_qpos, (S, K, dof), torch.float32, "grad_robot_qpos")
+            res["kp"] = new((S, K, N.NUM_KEYPOINTS, 3), "grad_keypoints")
+            res["fixed"] = new((S, K, nf), "grad_fixed_qpos") if nf else None
+            res["status"] = new((S, K), "status_out", torch.int32)
+
+        grads = dict(grad_last_qpos_out=grad_last_qpos_out, grad_window_qpos_out=grad_window_qpos_out,
+                     grad_window_keypoints_out=grad_window_keypoints_out,
+                     grad_window_fixed_qpos_out=grad_window_fixed_qpos_out)
+        g_last, g_wkp, g_wfix, g_wq = self._fixed_lag_vjp_call(state0, K, fill, False, smooth_weight, grads, stream,
+                                                               outputs)
+        return res["kp"], res["fixed"], g_last, g_wkp, g_wfix, g_wq, res["status"]
+
+    def flush_fixed_lag_vjp(self, state0: FixedLagState, *, grad_qpos=None, grad_robot_qpos=None, grad_last_qpos_out=None,
+                            grad_window_qpos_out=None, grad_window_keypoints_out=None, grad_window_fixed_qpos_out=None,
+                            stream=None):
+        """Backpropagation through `flush_fixed_lag` (the K = 0 form of `retarget_fixed_lag_vjp`): the flushed rows
+        (grad_qpos [S,L,opt_dof], grad_robot_qpos [S,L,dof]; rows past the count are ignored) are state0's held slots of
+        window_qpos, the last of them the new anchor.  Returns (grad_last_qpos, grad_window_keypoints,
+        grad_window_fixed_qpos or None, grad_window_qpos) of `state0`, the state before the flush."""
+        import torch
+
+        opt = self.optimizer
+        S, L = int(state0.last_qpos.shape[0]), int(state0.lag)
+        n, dof = opt.opt_dof, opt.robot.dof
+
+        def fill(io, chk, new):
+            if grad_qpos is not None:
+                io.grad_flush_qpos = chk(grad_qpos, (S, L, n), torch.float32, "grad_qpos")
+            if grad_robot_qpos is not None:
+                io.grad_flush_robot_qpos = chk(grad_robot_qpos, (S, L, dof), torch.float32, "grad_robot_qpos")
+
+        grads = dict(grad_last_qpos_out=grad_last_qpos_out, grad_window_qpos_out=grad_window_qpos_out,
+                     grad_window_keypoints_out=grad_window_keypoints_out,
+                     grad_window_fixed_qpos_out=grad_window_fixed_qpos_out)
+        return self._fixed_lag_vjp_call(state0, 0, fill, True, None, grads, stream)

@@ -581,6 +581,105 @@ size_t dexr_fixed_lag_workspace_bytes(const dexr_robot_t* robot, int64_t num_str
 int dexr_fixed_lag_step(const dexr_robot_t* robot, const dexr_params_t* params, const dexr_fixed_lag_t* io,
                         int64_t num_streams, int64_t num_ticks, void* cuda_stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Recording a fixed-lag call for its backward: dexr_fixed_lag_step_tape is dexr_fixed_lag_step that also stores, for tick k
+ * of stream s, the window minimiser X^k the tick's solve left (tape.qpos[s,k,0..m-1], m the window's length; rows m..L are
+ * not written) and the committed DexPilot flags that solve started from (tape.projected[s,k], DexPilot only; NULL
+ * otherwise).  Outputs and state are bit-identical with and without recording.  The tape holds S K (L+1) n_var floats:
+ * 84 MB at S = 256, K = 300, L = 16, n_var = 16.  Checks, workspace and asynchrony as dexr_fixed_lag_step.
+ * ------------------------------------------------------------------------------------------- */
+typedef struct dexr_fixed_lag_tape {
+  float* qpos;        /* [S,K,L+1,n_var] each tick's window minimiser                                                  */
+  uint8_t* projected; /* [S,K,len_proj] the committed flags each tick's solve started from (DexPilot), or NULL          */
+} dexr_fixed_lag_tape_t;
+size_t dexr_fixed_lag_tape_sizeof(void);
+int dexr_fixed_lag_step_tape(const dexr_robot_t* robot, const dexr_params_t* params, const dexr_fixed_lag_t* io,
+                             const dexr_fixed_lag_tape_t* tape, int64_t num_streams, int64_t num_ticks, void* cuda_stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * Backpropagation through fixed-lag smoothing: the VJP of one recorded dexr_fixed_lag_step_tape call (K ticks of lag L,
+ * optionally followed by a flush) with respect to its new frames and the state it started from, every stream in one launch.
+ * Per stream, with h0 = clamp(window_len, 0, L) held frames, the inputs are u_0 .. u_{h0+K-1} (the held frames, then the
+ * K new ones); c_k = max(0, h0 + k - L) frames are committed before tick k, which solves the window W_k = u_{c_k} ..
+ * u_{h0+k} for its minimiser X^k (tape.qpos[s,k]), anchored at A_k = last_qpos when c_k = 0 and at X^{k-1}[0] (the frame
+ * tick k-1 committed) otherwise.  A loss on the emitted rows, the flushed rows and the final state reaches the inputs only
+ * through the emitting windows' minimisers and the last tick's; every other solve only picks a basin and is not
+ * differentiated (as qpos_init is not in dexr_smooth_sequences_packed_vjp).  The backward walks k = K-1 .. 0 carrying abar,
+ * the cotangent of the current anchor:
+ *   1. the window cotangent: on an emitting tick slot 0 gets grad_qpos[k] + M^T grad_robot_qpos[k] + abar; the last tick
+ *      also takes the flushed rows' and the final state's cotangents (grad_last_qpos_out, the held slots of
+ *      grad_window_qpos_out), each at the slot it came from (shifted by one when the last tick emitted).  grad_last_qpos_out
+ *      goes to the last flushed frame when the call flushed held frames, else to X^{K-1}[0] when the last tick emitted,
+ *      else to last_qpos.  Cotangents on PENDING rows, and on flush rows past flush_count, are ignored;
+ *   2. W_k is differentiated exactly as dexr_smooth_sequences_packed_vjp differentiates a clip (same active set, block
+ *      Thomas, target pass), at X^k, anchor A_k, the flags of tape.projected[s,k] and w = smooth_weight;
+ *   3. each window frame's keypoint and fixed-joint cotangent is added to the frame of the call it came from
+ *      (grad_keypoints[s,k'] for a new frame, grad_window_keypoints[s,j] for one held when the call started); the anchor
+ *      cotangent 2 w v_0 (where the clip passes) becomes abar, which feeds X^{k-1}[0] when c_k >= 1 and grad_last_qpos
+ *      when c_k = 0.
+ * Cotangents on the final state's window_keypoints / window_fixed_qpos (held slots only) go straight back to the input
+ * frames those slots hold, and start those frames' sums; the window contributions follow in decreasing tick order.  So a
+ * call split into chunks chained through the state cotangents gives the same bits as one call.  The incoming window_qpos is
+ * a warm start: its cotangent is 0 when K > 0.  With K = 0 a flush's rows ARE the incoming held slots of window_qpos (with
+ * the mimic fold; a fixed joint's share goes to grad_window_fixed_qpos), and K = 0 without a flush passes the state's
+ * cotangents through.
+ *   Per window, as in dexr_smooth_sequences_packed_vjp: a window whose stacked free Hessian is not positive definite
+ *     contributes zero and cuts the anchor chain (its emitting tick gets DEXR_STATUS_NOT_PD); a non-finite point, anchor or
+ *     cotangent makes everything the window writes NaN (DEXR_STATUS_NONFINITE), which reaches earlier ticks through abar;
+ *     a missing frame gets zero cotangents but carries the chain.  One difference: a flushed row's robot_qpos cotangent on
+ *     a fixed joint is that joint's direct term, added to the frame's sum before the windows (so that chunks stay
+ *     bit-identical), and it is kept where dexr_smooth_sequences_packed_vjp zeroes its direct term: on a NOT_PD window and
+ *     on a missing frame.  Without those, L >= K - 1 with a flush gives the smoother VJP's bits on the whole clip.
+ *   status_out[s,k]: the emitted frame's window status (0, NOT_PD or NONFINITE, | MISSING) on emitting ticks,
+ *     DEXR_STATUS_PENDING on the others.
+ * Not differentiated: the DexPilot flags, w, the starting trajectories.  Raw landmarks (params.preprocess != 0) are refused.
+ * last_qpos and window_len must be the state before the call; keypoints, fixed_qpos and the tape the call's own;
+ * `projected` and `window_qpos` are not read (the flags come from the tape, the warm start gets no derivative).
+ * Every output is written in full (zeros where nothing reaches): grad_keypoints / grad_fixed_qpos [S,K,...], the
+ * grad_window_* [S,L+1,...], grad_last_qpos [S,n_var].  Every cotangent input and every output but grad_keypoints (when
+ * K > 0) may be NULL.  `workspace`: at least dexr_fixed_lag_vjp_workspace_bytes(robot, num_streams, lag) bytes
+ * (DEXR_E_INVALID below): one rebuilt window per stream.  Asynchronous on `cuda_stream`, allocates nothing, does nothing for
+ * num_streams == 0.  All pointers are DEVICE pointers.
+ * ------------------------------------------------------------------------------------------- */
+typedef struct dexr_fixed_lag_vjp {
+  /* the forward's inputs and the state before the call */
+  const float* keypoints;             /* [S,K,21,3] as given to the forward                                           */
+  const float* fixed_qpos;            /* [S,K,n_fixed] or NULL when n_fixed == 0                                      */
+  const float* last_qpos;             /* [S,n_var] the anchor before the call                                         */
+  const uint8_t* projected;           /* [S,len_proj] the flags before the call (not read: the tape holds each tick's) */
+  const float* window_keypoints;      /* [S,L+1,21,3] before the call                                                 */
+  const float* window_fixed_qpos;     /* [S,L+1,n_fixed] before the call, or NULL                                     */
+  const float* window_qpos;           /* [S,L+1,n_var] before the call (not read: a warm start)                       */
+  const int32_t* window_len;          /* [S] before the call                                                          */
+  dexr_fixed_lag_tape_t tape;         /* the call's recording                                                         */
+  /* cotangents (NULL = 0) */
+  const float* grad_qpos;             /* [S,K,n_var] of qpos_out                                                      */
+  const float* grad_robot_qpos;       /* [S,K,dof] of robot_qpos_out                                                  */
+  const float* grad_flush_qpos;       /* [S,L,n_var] of flush_qpos_out                                                */
+  const float* grad_flush_robot_qpos; /* [S,L,dof] of flush_robot_qpos_out                                            */
+  const float* grad_last_qpos_out;    /* [S,n_var] of the final last_qpos                                             */
+  const float* grad_window_qpos_out;  /* [S,L+1,n_var] of the final window_qpos (held slots read)                     */
+  const float* grad_window_keypoints_out;  /* [S,L+1,21,3] of the final window_keypoints (held slots read)            */
+  const float* grad_window_fixed_qpos_out; /* [S,L+1,n_fixed] of the final window_fixed_qpos (held slots read)        */
+  /* outputs (NULL: not written; grad_keypoints is required when K > 0) */
+  float* grad_keypoints;              /* [S,K,21,3]                                                                   */
+  float* grad_fixed_qpos;             /* [S,K,n_fixed]                                                                */
+  float* grad_last_qpos;              /* [S,n_var] of the incoming anchor                                             */
+  float* grad_window_keypoints;       /* [S,L+1,21,3] of the incoming held frames                                     */
+  float* grad_window_fixed_qpos;      /* [S,L+1,n_fixed]                                                              */
+  float* grad_window_qpos;            /* [S,L+1,n_var] (0 when K > 0)                                                 */
+  int32_t* status_out;                /* [S,K]                                                                        */
+  int32_t lag;
+  int32_t flushed;                    /* non-zero: the forward flushed after its ticks (flush_count_out non-NULL)     */
+  float smooth_weight;                /* as given to the forward; < 0: params.norm_delta                              */
+  void* workspace;                    /* >= dexr_fixed_lag_vjp_workspace_bytes(robot, S, lag) bytes                   */
+  size_t workspace_bytes;
+} dexr_fixed_lag_vjp_t;
+size_t dexr_fixed_lag_vjp_sizeof(void);
+size_t dexr_fixed_lag_vjp_workspace_bytes(const dexr_robot_t* robot, int64_t num_streams, int32_t lag);
+int dexr_fixed_lag_step_vjp(const dexr_robot_t* robot, const dexr_params_t* params, const dexr_fixed_lag_vjp_t* io,
+                            int64_t num_streams, int64_t num_ticks, void* cuda_stream);
+
 #ifdef __cplusplus
 }
 #endif
