@@ -203,7 +203,8 @@ EXPORTS = [
     "dexr_smooth_sizeof", "dexr_smooth_workspace_bytes", "dexr_smooth_sequences_packed", "dexr_smooth_vjp_sizeof",
     "dexr_smooth_sequences_packed_vjp", "dexr_fixed_lag_sizeof", "dexr_fixed_lag_workspace_bytes", "dexr_fixed_lag_step",
     "dexr_fixed_lag_tape_sizeof", "dexr_fixed_lag_step_tape", "dexr_fixed_lag_vjp_sizeof",
-    "dexr_fixed_lag_vjp_workspace_bytes", "dexr_fixed_lag_step_vjp",
+    "dexr_fixed_lag_vjp_workspace_bytes", "dexr_fixed_lag_step_vjp", "dexr_smooth_accel_workspace_bytes",
+    "dexr_smooth_sequences_packed_accel", "dexr_smooth_sequences_packed_accel_vjp",
 ]
 
 _LIB = None
@@ -322,6 +323,17 @@ def load():
             raise DexrError("dexr_smooth_vjp_t layout mismatch between library and binding (stale DEXR_LIBRARY?)")
         lib.dexr_smooth_sequences_packed_vjp.argtypes = [C.c_void_p, C.POINTER(DexrParams), C.POINTER(DexrSmoothVjp),
                                                          C.c_void_p, C.c_int64, C.c_int64, C.c_void_p]
+    if hasattr(lib, "dexr_smooth_sequences_packed_accel"):
+        lib.dexr_smooth_accel_workspace_bytes.argtypes = [C.c_void_p, C.c_int64]
+        lib.dexr_smooth_accel_workspace_bytes.restype = C.c_size_t
+        lib.dexr_smooth_sequences_packed_accel.argtypes = [C.c_void_p, C.POINTER(DexrParams), C.POINTER(DexrSmooth), _f,
+                                                           C.c_void_p, C.c_int64, C.c_int64, C.c_void_p]
+        lib.dexr_smooth_sequences_packed_accel_vjp.argtypes = [C.c_void_p, C.POINTER(DexrParams),
+                                                               C.POINTER(DexrSmoothVjp), _f, C.c_void_p, C.c_int64,
+                                                               C.c_int64, C.c_void_p]
+    elif not os.environ.get("DEXR_LIBRARY"):
+        raise DexrError(f"{path} does not export dexr_smooth_sequences_packed_accel: rebuild it "
+                        "(python -m dex_retargeting_b200.build --force)")
     elif not os.environ.get("DEXR_LIBRARY"):
         raise DexrError(f"{path} does not export dexr_smooth_vjp_sizeof: rebuild it "
                         "(python -m dex_retargeting_b200.build --force)")

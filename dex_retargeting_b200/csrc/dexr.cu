@@ -703,6 +703,42 @@ __global__ void __launch_bounds__(kEvalWarps * 32, G == 16 ? 2 : 1) dexr_smooth_
     smooth_vjp_packed_stream(sv, a.io, a.dm, pk, i, lane < G);
 }
 
+// the acceleration-penalised smoother and its backpropagation: dexr_smooth_kernel's and dexr_smooth_vjp_kernel's launch
+// shapes and stream slots, running smooth_packed_stream<G, true> and smooth_vjp_packed_stream<G, true> (their own kernels, so
+// the velocity-only ones keep their code); a.io.smooth_weight holds the acceleration weight c
+template <int G>
+__global__ void __launch_bounds__(kEvalWarps * 32, G == 16 ? 2 : 1) dexr_smooth_accel_kernel(const SmoothArgs a,
+                                                                                             const PackedLayout pk) {
+  load_shared_table(*reinterpret_cast<SharedTable*>(dsmem), a.table);
+  __syncthreads();
+  constexpr int GPW = 32 / G;
+  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
+  const int lane = threadIdx.x & 31;
+  const int gid = warp * GPW + lane / G;
+  Solver<G, 0> sv;
+  sv.init(a.table, a.dm, (uint32_t)(a.scratch_off + gid * VjpScratch<G>::kFloats * 4), a.prm, lane);
+  float* const ws = static_cast<float*>(a.io.workspace);
+  for (long long base = 0; base < a.S; base += (long long)gridDim.x * kEvalWarps) {
+    const PackedStream ps = packed_stream(pk, base + (long long)warp * gridDim.x + blockIdx.x);
+    smooth_packed_stream<G, true>(sv, a.io, a.dm, a.prm, ps, lane < G, ws);
+  }
+}
+
+template <int G>
+__global__ void __launch_bounds__(kEvalWarps * 32, G == 16 ? 2 : 1) dexr_smooth_accel_vjp_kernel(const SmoothVjpArgs a,
+                                                                                                 const PackedLayout pk) {
+  load_shared_table(*reinterpret_cast<SharedTable*>(dsmem), a.table);
+  __syncthreads();
+  constexpr int GPW = 32 / G;
+  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
+  const int lane = threadIdx.x & 31;
+  const int gid = warp * GPW + lane / G;
+  Solver<G, 0> sv;
+  sv.init(a.table, a.dm, (uint32_t)(a.scratch_off + gid * VjpScratch<G>::kFloats * 4), a.prm, lane);
+  for (long long i = (long long)warp * gridDim.x + blockIdx.x; i < a.S; i += (long long)gridDim.x * kEvalWarps)
+    smooth_vjp_packed_stream<G, true>(sv, a.io, a.dm, pk, i, lane < G);
+}
+
 // fixed-lag smoothing of live streams: dexr_smooth_kernel's launch shape and stream slots, K ticks of one stream per warp
 // (fixed_lag_tick; a 16-lane warp's second group idles)
 struct FixedLagArgs {
@@ -1988,6 +2024,35 @@ static int launch_smooth(dexr_robot* r, const dexr_params_t* prm, const dexr_smo
   return 0;
 }
 
+// dexr_smooth_sequences_packed_accel: launch_smooth's CTA and occupancy rule.
+template <int G>
+static int launch_smooth_accel(dexr_robot* r, const dexr_params_t* prm, const dexr_smooth_t* io, float accel,
+                               const PackedLayout& pk, cudaStream_t stream) {
+  SmoothArgs a{};
+  a.table = r->table_dev;
+  a.prm = *prm;
+  if (!(io->smooth_weight < 0.f)) a.prm.norm_delta = io->smooth_weight;
+  a.io = *io;
+  a.io.smooth_weight = accel;  // (w is in a.prm.norm_delta)
+  a.S = pk.S;
+  a.dm = make_dims(r->host);
+  a.scratch_off = round_up((int)sizeof(SharedTable), 16);
+  constexpr int GPW = 32 / G;
+  const int smem = a.scratch_off + kEvalWarps * GPW * VjpScratch<G>::kFloats * 4;
+  auto kern = dexr_smooth_accel_kernel<G>;
+  CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  int per_sm = 1;
+  if (int e = eval_ctas_per_sm(kern, smem, &per_sm)) return e;
+  const int grid = (int)std::min<long long>(pk.S, (long long)r->num_sms * per_sm);
+  kern<<<grid, kEvalWarps * 32, smem, stream>>>(a, pk);
+  CUDA_TRY(cudaGetLastError());
+  {
+    std::lock_guard<std::mutex> lk(r->info_mu);
+    r->last = dexr_launch_info_t{grid, kEvalWarps * 32, smem, 0, G, kEvalWarps, r->last.kernels_launched + 1};
+  }
+  return 0;
+}
+
 extern "C" size_t dexr_smooth_sizeof(void) { return sizeof(dexr_smooth_t); }
 
 extern "C" size_t dexr_smooth_workspace_bytes(const dexr_robot_t* robot, int64_t num_frames) {
@@ -2037,6 +2102,35 @@ static int launch_smooth_vjp(dexr_robot* r, const dexr_params_t* prm, const dexr
   return 0;
 }
 
+// dexr_smooth_sequences_packed_accel_vjp: launch_smooth's CTA and occupancy rule.
+template <int G>
+static int launch_smooth_accel_vjp(dexr_robot* r, const dexr_params_t* prm, const dexr_smooth_vjp_t* io, float accel,
+                                   const PackedLayout& pk, cudaStream_t stream) {
+  SmoothVjpArgs a{};
+  a.table = r->table_dev;
+  a.prm = *prm;
+  if (!(io->smooth_weight < 0.f)) a.prm.norm_delta = io->smooth_weight;
+  a.io = *io;
+  a.io.smooth_weight = accel;  // (w is in a.prm.norm_delta)
+  a.S = pk.S;
+  a.dm = make_dims(r->host);
+  a.scratch_off = round_up((int)sizeof(SharedTable), 16);
+  constexpr int GPW = 32 / G;
+  const int smem = a.scratch_off + kEvalWarps * GPW * VjpScratch<G>::kFloats * 4;
+  auto kern = dexr_smooth_accel_vjp_kernel<G>;
+  CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  int per_sm = 1;
+  if (int e = eval_ctas_per_sm(kern, smem, &per_sm)) return e;
+  const int grid = (int)std::min<long long>(pk.S, (long long)r->num_sms * per_sm);
+  kern<<<grid, kEvalWarps * 32, smem, stream>>>(a, pk);
+  CUDA_TRY(cudaGetLastError());
+  {
+    std::lock_guard<std::mutex> lk(r->info_mu);
+    r->last = dexr_launch_info_t{grid, kEvalWarps * 32, smem, 0, G, kEvalWarps, r->last.kernels_launched + 1};
+  }
+  return 0;
+}
+
 extern "C" size_t dexr_smooth_vjp_sizeof(void) { return sizeof(dexr_smooth_vjp_t); }
 
 extern "C" int dexr_smooth_sequences_packed_vjp(const dexr_robot_t* robot, const dexr_params_t* params,
@@ -2053,6 +2147,50 @@ extern "C" int dexr_smooth_sequences_packed_vjp(const dexr_robot_t* robot, const
   const PackedLayout pk{offsets, num_streams, num_frames};
   return eval_lanes(r->host) == 16 ? launch_smooth_vjp<16>(r, params, io, pk, stream)
                                    : launch_smooth_vjp<32>(r, params, io, pk, stream);
+}
+
+extern "C" size_t dexr_smooth_accel_workspace_bytes(const dexr_robot_t* robot, int64_t num_frames) {
+  return robot ? smooth_accel_workspace_bytes(robot->host, num_frames) : 0;
+}
+
+extern "C" int dexr_smooth_sequences_packed_accel(const dexr_robot_t* robot, const dexr_params_t* params,
+                                                  const dexr_smooth_t* io, float accel_weight, const int64_t* offsets,
+                                                  int64_t num_streams, int64_t num_frames, void* cuda_stream) {
+  if (!robot || !params || !io) return fail(DEXR_E_INVALID, "dexr_smooth_sequences_packed_accel: null argument");
+  if (accel_weight == 0.f)
+    return dexr_smooth_sequences_packed(robot, params, io, offsets, num_streams, num_frames, cuda_stream);
+  if (const char* msg = smooth_io_error(robot->host, *io, *params, offsets, num_streams, num_frames))
+    return fail(DEXR_E_INVALID, "%s", msg);
+  if (const char* msg = smooth_accel_error(robot->host, accel_weight, io->workspace, io->workspace_bytes, num_frames))
+    return fail(DEXR_E_INVALID, "%s", msg);
+  if (int e = check_params(params)) return e;
+  if (num_streams == 0 || num_frames == 0) return 0;
+  DEVICE_SCOPE(robot->device);
+  dexr_robot* r = const_cast<dexr_robot*>(robot);
+  cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
+  const PackedLayout pk{offsets, num_streams, num_frames};
+  return eval_lanes(r->host) == 16 ? launch_smooth_accel<16>(r, params, io, accel_weight, pk, stream)
+                                   : launch_smooth_accel<32>(r, params, io, accel_weight, pk, stream);
+}
+
+extern "C" int dexr_smooth_sequences_packed_accel_vjp(const dexr_robot_t* robot, const dexr_params_t* params,
+                                                      const dexr_smooth_vjp_t* io, float accel_weight, const int64_t* offsets,
+                                                      int64_t num_streams, int64_t num_frames, void* cuda_stream) {
+  if (!robot || !params || !io) return fail(DEXR_E_INVALID, "dexr_smooth_sequences_packed_accel_vjp: null argument");
+  if (accel_weight == 0.f)
+    return dexr_smooth_sequences_packed_vjp(robot, params, io, offsets, num_streams, num_frames, cuda_stream);
+  if (const char* msg = smooth_vjp_io_error(robot->host, *io, *params, offsets, num_streams, num_frames))
+    return fail(DEXR_E_INVALID, "%s", msg);
+  if (const char* msg = smooth_accel_error(robot->host, accel_weight, io->workspace, io->workspace_bytes, num_frames))
+    return fail(DEXR_E_INVALID, "%s", msg);
+  if (int e = check_loss_params(params)) return e;
+  if (num_streams == 0 || num_frames == 0) return 0;
+  DEVICE_SCOPE(robot->device);
+  dexr_robot* r = const_cast<dexr_robot*>(robot);
+  cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
+  const PackedLayout pk{offsets, num_streams, num_frames};
+  return eval_lanes(r->host) == 16 ? launch_smooth_accel_vjp<16>(r, params, io, accel_weight, pk, stream)
+                                   : launch_smooth_accel_vjp<32>(r, params, io, accel_weight, pk, stream);
 }
 
 // dexr_fixed_lag_step: launch_smooth's CTA and occupancy rule.

@@ -2654,6 +2654,21 @@ struct SmoothWs {
   static constexpr int kFloats = kG + G;
 };
 
+// The workspace of the acceleration-penalised smoother (dexr_smooth_sequences_packed_accel, DESIGN.md 3.16): SmoothWs<G>
+// followed by
+//   kE  [G][G] E_t, the dense coupling block between frames t and t+1 that the banded elimination leaves: entry [k][c]
+//              (row k: frame t's joint, column c: frame t+1's) at k * G + c, written by lane c
+template <int G>
+struct SmoothAccWs : SmoothWs<G> {
+  static constexpr int kE = SmoothWs<G>::kFloats;
+  static constexpr int kFloats = kE + G * G;
+};
+
+template <int G, bool ACC>
+struct SmoothWsOf { using type = SmoothWs<G>; };
+template <int G>
+struct SmoothWsOf<G, true> { using type = SmoothAccWs<G>; };
+
 // Relative resolution of F in the smoother's acceptance test: a trial whose change of F, and whose predicted decrease
 // -g.delta / 2, both lie within kSmoothNoise F is accepted.  Near the minimiser the decrease a Newton step brings along a
 // flat direction (a joint the keypoints hardly determine) is far below what the fp32 terms resolve; rejecting it there
@@ -2666,6 +2681,22 @@ constexpr float kSmoothMuMax = 1e12f;
 inline size_t smooth_workspace_bytes(const dexr_table_t& t, long long num_frames) {
   const int floats = eval_lanes(t) == 16 ? SmoothWs<16>::kFloats : SmoothWs<32>::kFloats;
   return num_frames > 0 ? (size_t)num_frames * (size_t)floats * sizeof(float) : 0;
+}
+
+// Bytes of workspace an acceleration-penalised call on `num_frames` frames needs (dexr_smooth_accel_workspace_bytes).
+inline size_t smooth_accel_workspace_bytes(const dexr_table_t& t, long long num_frames) {
+  const int floats = eval_lanes(t) == 16 ? SmoothAccWs<16>::kFloats : SmoothAccWs<32>::kFloats;
+  return num_frames > 0 ? (size_t)num_frames * (size_t)floats * sizeof(float) : 0;
+}
+
+// The extra argument checks of the acceleration-penalised entry points (after smooth_io_error / smooth_vjp_io_error):
+// nullptr, or what is wrong.
+inline const char* smooth_accel_error(const dexr_table_t& t, float accel_weight, const void* workspace,
+                                      size_t workspace_bytes, long long N) {
+  if (!(accel_weight >= 0.f && accel_weight <= 3.0e38f)) return "accel_weight must be finite and >= 0";
+  if (N > 0 && (!workspace || workspace_bytes < smooth_accel_workspace_bytes(t, N)))
+    return "workspace smaller than dexr_smooth_accel_workspace_bytes(robot, num_frames)";
+  return nullptr;
 }
 
 // The argument checks of dexr_smooth_sequences_packed: nullptr, or what is wrong.  Host code shared by the library and the
@@ -2743,14 +2774,108 @@ __device__ __forceinline__ void smooth_reset_flags(const Solver<G, 0>& sv, const
   __syncwarp();
 }
 
+// The acceleration-penalised smoother's coefficients at frame t of a stream of `len` frames (DESIGN.md 3.16): the triples
+// (s-1, s, s+1) of F_c have centres s in [anchor ? 0 : 1, len - 2], the clipped anchor standing in for frame -1.  Frame t is
+// the right end of the triple centred at t-1 (`right`), the centre of the one at t (`centre`) and the left end of the one at
+// t+1 (`left`).  Group-uniform.
+struct AccTerms {
+  bool right, centre, left;
+  __device__ __forceinline__ AccTerms(int t, int len, bool anchor)
+      : right(t >= 2 || (t == 1 && anchor)), centre((t >= 1 || anchor) && t + 1 < len), left(t + 2 < len) {}
+  // m_t: the sum of the squared coefficients (1, -2, 1) of frame t over its triples
+  __device__ __forceinline__ float diag() const { return (right ? 1.f : 0.f) + (centre ? 4.f : 0.f) + (left ? 1.f : 0.f); }
+  // the number of triples that hold both t and t+1
+  __device__ __forceinline__ float pair() const { return (centre ? 1.f : 0.f) + (left ? 1.f : 0.f); }
+  // d/dx_t of c times the triples' squares, from x_{t-2} .. x_{t+2} (x_{-1}: the anchor; entries of absent frames unused)
+  __device__ __forceinline__ float grad(float c, float xp2, float xp, float x, float xn, float xn2) const {
+    const float sr = x - 2.f * xp + xp2, sc = xn - 2.f * x + xp, sl = xn2 - 2.f * xn + x;
+    return 2.f * c * ((right ? sr : 0.f) - (centre ? 2.f * sc : 0.f) + (left ? sl : 0.f));
+  }
+  // F_t's share of c times the triples' squares: the triple centred at t-1
+  __device__ __forceinline__ float cost(float c, float xp2, float xp, float x) const {
+    const float sr = x - 2.f * xp + xp2;
+    return right ? c * sr * sr : 0.f;
+  }
+};
+
+// The banded block elimination's share of frame t (ACC), between fold_free_block and factor_rows: with the dense coupling
+// E_{t-1} between frames t-1 and t and P = Z_{t-1} E_{t-1} (column per lane, in the kH area),
+//   S_t = D_t - E_{t-1}^T P - c2^2 Z_{t-2},   y_t = y - P^T y_{t-1} - c2 Z_{t-2} y_{t-2},   E_t = b I - c1 P^T
+// where b is the Hessian's scalar block between t and t+1, c1 the one between t-1 and t+1 and c2 the one between t-2 and t.
+// `wt`: frame t's workspace (frames t-1 and t-2 before it; read only while `live`, which holds for them whenever it holds for
+// t); `yp1`: this lane's y_{t-1} (y_{t-2} is read back from the workspace).  Z_{t-1}, Z_{t-2} are zero off their free
+// variables, and the caller's A and y are only touched on frame t's, so the elimination is that of the free subproblem.
+// E_t goes to the workspace; returns y_t.
+template <int G, class W>
+__device__ __forceinline__ float accel_eliminate(const Solver<G, 0>& sv, int dof, float* A, float* wt, int t, bool live,
+                                                 bool free_, unsigned fmask, float y, float yp1, float b, float c1, float c2) {
+  constexpr int NP = G;
+  const int l = sv.l;
+  const bool joint = l < dof;
+  float* const P = sv.scf() + VjpScratch<G>::kH;
+  const float* const zp = wt - W::kFloats + W::kZ;
+  const float* const ep = wt - W::kFloats + W::kE;
+  __syncwarp();  // fold_free_block has read H_q from the kH area (other lanes' columns, with mimic joints)
+  if (t > 0) {  // (warp-uniform)
+    for (int i = 0; i < dof; ++i) {
+      float s = 0.f;
+      if (live && joint)
+        for (int k = 0; k < dof; ++k) s = fmaf(zp[i * G + k], ep[k * G + l], s);
+      P[i * NP + l] = s;
+    }
+    __syncwarp();
+    float py = 0.f;
+    for (int k = 0; k < dof; ++k) py = fmaf(P[k * NP + l], gshfl<G>(yp1, k), py);
+    if (free_) {
+      y -= py;
+      for (int c = 0; c < dof; ++c) {
+        if (!((fmask >> c) & 1u)) continue;
+        float s = 0.f;
+        for (int k = 0; k < dof; ++k) s = fmaf(ep[k * G + l], P[k * NP + c], s);
+        A[l * (NP + 1) + c] -= s;
+      }
+    }
+  }
+  if (t > 1) {  // (warp-uniform)
+    const float* const zq = zp - W::kFloats;
+    const float yp2 = live ? zq[W::kY - W::kZ + l] : 0.f;
+    float zy = 0.f;
+    for (int c = 0; c < dof; ++c) {
+      const float z = live ? zq[c * G + l] : 0.f;
+      zy = fmaf(z, gshfl<G>(yp2, c), zy);
+      if (free_ && ((fmask >> c) & 1u)) A[l * (NP + 1) + c] = fmaf(-c2 * c2, z, A[l * (NP + 1) + c]);
+    }
+    if (free_) y = fmaf(-c2, zy, y);
+  }
+  if (live)
+    for (int k = 0; k < dof; ++k) wt[W::kE + k * G + l] = (k == l ? b : 0.f) - ((t > 0 && joint) ? c1 * P[l * NP + k] : 0.f);
+  __syncwarp();  // the factorisation and the inverse rewrite A and the kH area
+  return y;
+}
+
+// The banded back substitution's right-hand side at frame t (ACC): y_t - E_t d_{t+1} - c2 d_{t+2} on this lane (`d1`: this
+// lane's entry of d_{t+1}; d_{t+2} is read back from slot D of frame t+2's workspace; `n1`, `n2`: whether those frames exist).
+template <int G, class W, int D>
+__device__ __forceinline__ float accel_back_rhs(const float* wt, int l, int dof, bool live, bool n1, bool n2, float d1,
+                                                float c2) {
+  float ed = 0.f;
+  for (int k = 0; k < dof; ++k) ed = fmaf((live && n1 && l < dof) ? wt[W::kE + l * G + k] : 0.f, gshfl<G>(d1, k), ed);
+  return live ? wt[W::kY + l] - ed - (n2 ? c2 * wt[2 * W::kFloats + D + l] : 0.f) : 0.f;
+}
+
 // One packed stream `ps` (ps.s < 0: none) of dexr_smooth_sequences_packed; `owner`: this group runs the stream (the kernel
 // gives a 16-lane warp's second group none).  The warp walks its groups' longer stream in every sweep and iterates until
 // every group is done; a group that is done, or past its stream's end, runs its frames inactive with its writes off.  `ws`: the workspace,
 // SmoothWs<G>::kFloats per frame.  `dm` and `prm` are the kernel argument's.
-template <int G>
+// ACC (dexr_smooth_sequences_packed_accel, DESIGN.md 3.16): F_c = F + c times the squared second differences of the
+// stream (the anchor as frame -1), a block-pentadiagonal Hessian eliminated by accel_eliminate / accel_back_rhs in place of
+// block Thomas, SmoothAccWs<G>::kFloats per frame; everything else as above.  c is io.smooth_weight: the launch has moved w
+// into sv.prm.norm_delta, and c travels in the io rather than in a parameter of its own, which would change the code of the
+// velocity-only instantiation.
+template <int G, bool ACC = false>
 __device__ __forceinline__ void smooth_packed_stream(Solver<G, 0>& sv, const dexr_smooth_t& io, const Dims& dm,
                                                      const dexr_params_t& prm, const PackedStream& ps, bool owner, float* ws) {
-  using W = SmoothWs<G>;
+  using W = typename SmoothWsOf<G, ACC>::type;
   constexpr int NP = G;
   const SharedTable& st = Solver<G, 0>::ST();
   const int l = sv.l, lane = sv.lane, dof = dm.dof, n = dm.n_var;
@@ -2811,7 +2936,14 @@ __device__ __forceinline__ void smooth_packed_stream(Solver<G, 0>& sv, const dex
       const float xp = (live && t > 0) ? wt[W::kX + cur * G + l - W::kFloats] : a;
       const float xn = (live && has_next) ? wt[W::kX + cur * G + l + W::kFloats] : 0.f;
       const float v = smooth_eval(sv, io, dm, fr, x, xp, has_prev, missing, live);
-      if (live) {
+      if constexpr (ACC) {  // with the triples' share of F_t
+        const float xp2 = (live && t > 1) ? wt[W::kX + cur * G + l - 2 * W::kFloats] : a;
+        const float va = isvar ? v + AccTerms(t, len, anchor).cost(io.smooth_weight, xp2, xp, x) : v;
+        if (live) {
+          wt[W::kV + l] = va;
+          fsum += va;
+        }
+      } else if (live) {
         wt[W::kV + l] = v;
         fsum += v;
       }
@@ -2822,13 +2954,27 @@ __device__ __forceinline__ void smooth_packed_stream(Solver<G, 0>& sv, const dex
         for (int i = 0; i < NP; ++i) hq[i * NP + l] = 0.f;
       }
       g = isvar ? g + (has_prev ? w2 * (x - xp) : 0.f) + (has_next ? w2 * (x - xn) : 0.f) : 0.f;
+      if constexpr (ACC) {  // the triples' share of g_t
+        const AccTerms at(t, len, anchor);
+        const float xp2 = (live && t > 1) ? wt[W::kX + cur * G + l - 2 * W::kFloats] : a;
+        const float xn2 = (live && at.left) ? wt[W::kX + cur * G + l + 2 * W::kFloats] : 0.f;
+        if (isvar) g += at.grad(io.smooth_weight, xp2, xp, x, xn, xn2);
+      }
       const bool at_bound = isvar && ((x <= sv.lo && g > -kGradNoise) || (x >= sv.hi && g < kGradNoise));
       const bool free_ = live && isvar && !at_bound;
       const unsigned fmask = gballot<G>(free_, lane);
       __syncwarp();
-      fold_free_block(sv, dm, A, free_, fmask, fmaf(w2, (float)((has_prev ? 1 : 0) + (has_next ? 1 : 0)), mu));
+      if constexpr (ACC)
+        fold_free_block(sv, dm, A, free_, fmask, fmaf(2.f * io.smooth_weight, AccTerms(t, len, anchor).diag(),
+                                                      fmaf(w2, (float)((has_prev ? 1 : 0) + (has_next ? 1 : 0)), mu)));
+      else
+        fold_free_block(sv, dm, A, free_, fmask, fmaf(w2, (float)((has_prev ? 1 : 0) + (has_next ? 1 : 0)), mu));
       float y = free_ ? -g : 0.f;
-      if (t > 0) {  // (warp-uniform) the Schur complement of frame t - 1: Z_{t-1} is zero off its free variables
+      if constexpr (ACC)
+        y = accel_eliminate<G, W>(sv, dof, A, wt, t, live, free_, fmask, y, yprev,
+                                  -fmaf(4.f * io.smooth_weight, AccTerms(t, len, anchor).pair(), w2),
+                                  (t >= 1 && has_next) ? 2.f * io.smooth_weight : 0.f, 2.f * io.smooth_weight);
+      if (!ACC && t > 0) {  // (warp-uniform) the Schur complement of frame t - 1: Z_{t-1} is zero off its free variables
         const float* zp = wt - W::kFloats + W::kZ;
         float zy = 0.f;
         for (int c = 0; c < dof; ++c) {
@@ -2878,7 +3024,10 @@ __device__ __forceinline__ void smooth_packed_stream(Solver<G, 0>& sv, const dex
       const bool live = go && t < len;
       const int tc = t < tlast ? t : tlast;
       float* const wt = wsf + tc * W::kFloats;
-      const float r = live ? wt[W::kY + l] + (t + 1 < len ? w2 * dn : 0.f) : 0.f;
+      float r;
+      if constexpr (ACC)
+        r = accel_back_rhs<G, W, W::kY>(wt, l, dof, live, t + 1 < len, t + 2 < len, dn, 2.f * io.smooth_weight);
+      else r = live ? wt[W::kY + l] + (t + 1 < len ? w2 * dn : 0.f) : 0.f;
       float d = 0.f;
       for (int c = 0; c < dof; ++c) d = fmaf(live ? wt[W::kZ + c * G + l] : 0.f, gshfl<G>(r, c), d);
       if (live) {
@@ -2886,6 +3035,7 @@ __device__ __forceinline__ void smooth_packed_stream(Solver<G, 0>& sv, const dex
         wt[W::kX + (cur ^ 1) * G + l] = isvar ? fminf(fmaxf(x + d, sv.lo), sv.hi) : 0.f;
         smax = fmaxf(smax, fabsf(d));
         gd = fmaf(wt[W::kG + l], d, gd);
+        if constexpr (ACC) wt[W::kY + l] = d;  // (y_t is used up: d_t for frame t-2's right-hand side)
         dn = d;
       }
     }
@@ -2903,7 +3053,14 @@ __device__ __forceinline__ void smooth_packed_stream(Solver<G, 0>& sv, const dex
       const float x = wt[W::kX + (cur ^ 1) * G + l];
       const float xp = (live && t > 0) ? wt[W::kX + (cur ^ 1) * G + l - W::kFloats] : a;
       const float v = smooth_eval(sv, io, dm, fr, x, xp, t > 0 || anchor, missing, live);
-      if (live) {
+      if constexpr (ACC) {  // with the triples' share of F_t
+        const float xp2 = (live && t > 1) ? wt[W::kX + (cur ^ 1) * G + l - 2 * W::kFloats] : a;
+        const float va = isvar ? v + AccTerms(t, len, anchor).cost(io.smooth_weight, xp2, xp, x) : v;
+        if (live) {
+          dsum += va - wt[W::kV + l];
+          fnew += va;
+        }
+      } else if (live) {
         dsum += v - wt[W::kV + l];
         fnew += v;
       }
@@ -2978,10 +3135,13 @@ inline const char* smooth_vjp_io_error(const dexr_table_t& t, const dexr_smooth_
 //   cotangent the frame again (targets, FK, H_q), then vjp_tail's target pass and fixed-joint term with v_t.
 // The stream's NONFINITE and NOT_PD verdicts are known after the forward sweep and select every output.  `dm` and `ws` as in
 // smooth_packed_stream; sv.prm.norm_delta holds w.
-template <int G>
+// ACC (dexr_smooth_sequences_packed_accel_vjp): the exact block-pentadiagonal Hessian of F_c (c = io.smooth_weight, as in
+// smooth_packed_stream<G, true>), eliminated as the forward eliminates it with mu = 0; the anchor's cotangent gains
+// 4c v_0 - 2c v_1 when the stream has a second frame.
+template <int G, bool ACC = false>
 __device__ __forceinline__ void smooth_vjp_packed_stream(Solver<G, 0>& sv, const dexr_smooth_vjp_t& io, const Dims& dm,
                                                          const PackedLayout& pk, long long si, bool owner) {
-  using W = SmoothWs<G>;
+  using W = typename SmoothWsOf<G, ACC>::type;
   constexpr int NP = G;
   const SharedTable& st = Solver<G, 0>::ST();
   const int l = sv.l, lane = sv.lane, dof = dm.dof, n = dm.n_var;
@@ -3063,13 +3223,31 @@ __device__ __forceinline__ void smooth_vjp_packed_stream(Solver<G, 0>& sv, const
       for (int i = 0; i < NP; ++i) hq[i * NP + l] = 0.f;
     }
     g = isvar ? g + gs : 0.f;
+    if constexpr (ACC) {  // the triples' share of g_t (x_{-1}: the clipped anchor)
+      const AccTerms at(t, len, anchor);
+      float xp2 = t > 1 ? 0.f : clipped_anchor(), xn2 = 0.f, xn_ = 0.f;
+      if (live && isvar) {
+        if (t > 1) xp2 = io.qpos[(fr - 2) * n + sv.var];
+        if (has_next) xn_ = io.qpos[(fr + 1) * n + sv.var];
+        if (at.left) xn2 = io.qpos[(fr + 2) * n + sv.var];
+      }
+      if (isvar) g += at.grad(io.smooth_weight, xp2, xp, x, xn_, xn2);
+    }
     const bool at_bound = isvar && ((x <= sv.lo && g > -kGradNoise) || (x >= sv.hi && g < kGradNoise));
     const bool free_ = live && isvar && !at_bound;
     const unsigned fmask = gballot<G>(free_, lane);
     __syncwarp();
-    fold_free_block(sv, dm, A, free_, fmask, w2 * (float)((has_prev ? 1 : 0) + (has_next ? 1 : 0)));
+    if constexpr (ACC)
+      fold_free_block(sv, dm, A, free_, fmask, fmaf(2.f * io.smooth_weight, AccTerms(t, len, anchor).diag(),
+                                                    w2 * (float)((has_prev ? 1 : 0) + (has_next ? 1 : 0))));
+    else
+      fold_free_block(sv, dm, A, free_, fmask, w2 * (float)((has_prev ? 1 : 0) + (has_next ? 1 : 0)));
     float y = (free_ && live) ? wt[W::kG + l] : 0.f;
-    if (t > 0) {  // (warp-uniform) the Schur complement of frame t - 1: Z_{t-1} is zero off its free variables
+    if constexpr (ACC)
+      y = accel_eliminate<G, W>(sv, dof, A, wt, t, live, free_, fmask, y, yprev,
+                                -fmaf(4.f * io.smooth_weight, AccTerms(t, len, anchor).pair(), w2),
+                                (t >= 1 && has_next) ? 2.f * io.smooth_weight : 0.f, 2.f * io.smooth_weight);
+    if (!ACC && t > 0) {  // (warp-uniform) the Schur complement of frame t - 1: Z_{t-1} is zero off its free variables
       const float* zp = wt - W::kFloats + W::kZ;
       float zy = 0.f;
       for (int c = 0; c < dof; ++c) {
@@ -3107,7 +3285,10 @@ __device__ __forceinline__ void smooth_vjp_packed_stream(Solver<G, 0>& sv, const
     const bool live = t < len;
     const int tc = t < tlast ? t : tlast;
     float* const wt = static_cast<float*>(io.workspace) + (long long)(f0 + tc) * W::kFloats;
-    const float r = live ? wt[W::kY + l] + (t + 1 < len ? w2 * vn : 0.f) : 0.f;
+    float r;
+    if constexpr (ACC)
+      r = accel_back_rhs<G, W, W::kX>(wt, l, dof, live, t + 1 < len, t + 2 < len, vn, 2.f * io.smooth_weight);
+    else r = live ? wt[W::kY + l] + (t + 1 < len ? w2 * vn : 0.f) : 0.f;
     float d = 0.f;
     for (int c = 0; c < dof; ++c) d = fmaf(live ? wt[W::kZ + c * G + l] : 0.f, gshfl<G>(r, c), d);
     if (live) {
@@ -3158,7 +3339,13 @@ __device__ __forceinline__ void smooth_vjp_packed_stream(Solver<G, 0>& sv, const
     const float ar = raw_anchor();
     const bool passes = ar >= st.clip_lo[l] && ar <= st.clip_hi[l];
     const float v0 = has ? static_cast<const float*>(io.workspace)[(long long)f0 * W::kFloats + W::kX + l] : 0.f;
-    const float ga = nonfinite ? __int_as_float(0x7fc00000) : ((bad || !passes) ? 0.f : w2 * v0);
+    float ga = nonfinite ? __int_as_float(0x7fc00000) : ((bad || !passes) ? 0.f : w2 * v0);
+    if constexpr (ACC) {  // g_0 and g_1 also depend on a through the triple (a, x_0, x_1)
+      if (len > 1 && !nonfinite && !bad && passes) {
+        const float v1 = static_cast<const float*>(io.workspace)[(long long)(f0 + 1) * W::kFloats + W::kX + l];
+        ga = fmaf(2.f * io.smooth_weight, fmaf(2.f, v0, -v1), ga);
+      }
+    }
     io.grad_last_qpos[sc * n + sv.var] = has ? ga : 0.f;
   }
   __syncwarp();

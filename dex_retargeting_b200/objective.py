@@ -222,8 +222,8 @@ class _DifferentiableSmoothPackedSequences(torch.autograd.Function):
         view = StreamState(last_qpos=last0, filter_state=st.filter_state.detach(), filter_init=st.filter_init,
                            projected=proj0, damping=None if st.damping is None else st.damping.detach())
         rq, q, status = seq.smooth_packed_sequences(kp, layout, view, fixed_qpos=fixed, qpos_init=cfg["qpos_init"],
-                                                    smooth_weight=cfg["smooth_weight"])
-        ctx.seq, ctx.layout, ctx.smooth_weight = seq, layout, cfg["smooth_weight"]
+                                                    smooth_weight=cfg["smooth_weight"], accel_weight=cfg["accel_weight"])
+        ctx.seq, ctx.layout, ctx.smooth_weight, ctx.accel_weight = seq, layout, cfg["smooth_weight"], cfg["accel_weight"]
         ctx.save_for_backward(kp, fixed, last0, proj0, q)
         ctx.set_materialize_grads(False)
         ctx.mark_non_differentiable(status)
@@ -236,28 +236,31 @@ class _DifferentiableSmoothPackedSequences(torch.autograd.Function):
         c = (lambda g: None if g is None else g.contiguous())
         g_kp, g_fixed, g_last = ctx.seq.smooth_packed_sequences_vjp(
             kp, ctx.layout, q, last0, proj0, grad_qpos=c(g_q), grad_robot_qpos=c(g_rq), fixed_qpos=fixed,
-            smooth_weight=ctx.smooth_weight)
+            smooth_weight=ctx.smooth_weight, accel_weight=ctx.accel_weight)
         return g_kp, g_fixed, g_last, None, None
 
 
 def differentiable_smooth_packed_sequences(seq, keypoints, layout, state=None, fixed_qpos=None, *, qpos_init=None,
-                                           smooth_weight=None):
+                                           smooth_weight=None, accel_weight=None):
     """(robot_qpos [N,dof], qpos [N,opt_dof], status [N]) = `seq.smooth_packed_sequences(keypoints, layout, state, ...)`
     (recorded clips packed end to end, `seq.pack_streams`; float32 CUDA tensors as there), differentiable in `keypoints`
     [N,21,3], `fixed_qpos` [N,n_fixed] and the anchor `state.last_qpos` [S,opt_dof], through both robot_qpos and qpos.
     `state` (None: fresh streams) is read only, as by the forward.  backward() is one `smooth_packed_sequences_vjp`
     launch: the implicit-function derivative of the smoothed clips, one linear solve with the stacked Hessian per stream.
     The gradient is not causal: a loss on one frame reaches the keypoints of the whole clip.  The DexPilot flags, the
-    starting trajectory `qpos_init` and `smooth_weight` are not differentiated: they, and the state's other tensors, must
-    not require grad."""
+    starting trajectory `qpos_init`, `smooth_weight` and `accel_weight` (the acceleration penalty of
+    `smooth_packed_sequences`; None or 0: none) are not differentiated: they, and the state's other tensors, must not
+    require grad."""
     state = seq.make_stream_state(layout.num_streams) if state is None else state
-    for name, t in (("qpos_init", qpos_init), ("smooth_weight", smooth_weight), ("state.filter_state", state.filter_state),
-                    ("state.damping", state.damping)):
+    for name, t in (("qpos_init", qpos_init), ("smooth_weight", smooth_weight), ("accel_weight", accel_weight),
+                    ("state.filter_state", state.filter_state), ("state.damping", state.damping)):
         if isinstance(t, torch.Tensor) and t.requires_grad:
             raise ValueError(f"{name} requires grad, but the smoother is not differentiated in it: detach it")
     if isinstance(smooth_weight, torch.Tensor):
         smooth_weight = float(smooth_weight)
-    cfg = dict(state=state, layout=layout, qpos_init=qpos_init, smooth_weight=smooth_weight)
+    if isinstance(accel_weight, torch.Tensor):
+        accel_weight = float(accel_weight)
+    cfg = dict(state=state, layout=layout, qpos_init=qpos_init, smooth_weight=smooth_weight, accel_weight=accel_weight)
     return _DifferentiableSmoothPackedSequences.apply(keypoints, fixed_qpos, state.last_qpos, seq, cfg)
 
 

@@ -645,7 +645,8 @@ class SeqRetargeting:
         return g_kp, g_fixed, g_last, g_filter
 
     def smooth_packed_sequences(self, keypoints, layout: PackedStreams, state: Optional[StreamState] = None, *,
-                                fixed_qpos=None, qpos_init=None, smooth_weight=None, out=None, status_out=None, stream=None):
+                                fixed_qpos=None, qpos_init=None, smooth_weight=None, accel_weight=None, out=None,
+                                status_out=None, stream=None):
         """Offline smoothing of recorded clips (`dexr_smooth_sequences_packed`, one launch): every frame of each packed
         stream solved jointly, minimising sum_t L_t(x_t) + w sum_t |x_t - x_{t-1}|^2 + w |x_0 - clip(a)|^2 over the
         clip.  With w = norm_delta (`smooth_weight` None) this is the sum of the costs `retarget_packed_sequences` minimises
@@ -655,8 +656,10 @@ class SeqRetargeting:
         starting trajectory; None runs the taped `retarget_packed_sequences` on a copy of the state and starts from its
         tape.  A frame with a non-finite keypoint or fixed joint is filled in by the smoothness terms (STATUS_MISSING).
         Returns (robot_qpos [N,dof] (scatter + mimic, no low-pass filter), qpos [N,opt_dof], status [N] int32); a stream
-        whose status has STATUS_MAXITER returns its last accepted iterate (lower F than its start), not the minimiser.  Allocates
-        its workspace on the device; nothing is synchronised."""
+        whose status has STATUS_MAXITER returns its last accepted iterate (lower F than its start), not the minimiser.
+        `accel_weight` c > 0 adds c sum_t |x_{t+1} - 2 x_t + x_{t-1}|^2, the anchor counting as frame -1
+        (`dexr_smooth_sequences_packed_accel`): an acceleration penalty, which leaves constant-velocity motion alone; None
+        or 0 is the call above.  Allocates its workspace on the device; nothing is synchronised."""
         import torch
 
         opt = self.optimizer
@@ -693,20 +696,27 @@ class SeqRetargeting:
             status_out = torch.empty((N_,), dtype=torch.int32, device=dev)
         io.status_out = chk(status_out, (N_,), torch.int32, "status_out")
         io.smooth_weight = -1.0 if smooth_weight is None else float(smooth_weight)
-        nbytes = int(eng.lib.dexr_smooth_workspace_bytes(eng.handle, N_))
+        accel = 0.0 if accel_weight is None else float(accel_weight)
+        nbytes = int(eng.lib.dexr_smooth_accel_workspace_bytes(eng.handle, N_) if accel != 0.0
+                     else eng.lib.dexr_smooth_workspace_bytes(eng.handle, N_))
         ws = torch.empty((max(nbytes, 4),), dtype=torch.uint8, device=dev)
         io.workspace, io.workspace_bytes = ws.data_ptr(), nbytes
         s = stream if stream is not None else torch.cuda.current_stream(dev)
         p = opt.params(clip_init=True, lp_alpha=self.low_pass_alpha)
-        N.check(eng.lib.dexr_smooth_sequences_packed(eng.handle, C.byref(p), C.byref(io), C.c_void_p(offsets), S, N_,
-                                                     C.c_void_p(s.cuda_stream)), "dexr_smooth_sequences_packed")
+        if accel != 0.0:
+            N.check(eng.lib.dexr_smooth_sequences_packed_accel(eng.handle, C.byref(p), C.byref(io), accel, C.c_void_p(offsets),
+                                                               S, N_, C.c_void_p(s.cuda_stream)),
+                    "dexr_smooth_sequences_packed_accel")
+        else:
+            N.check(eng.lib.dexr_smooth_sequences_packed(eng.handle, C.byref(p), C.byref(io), C.c_void_p(offsets), S, N_,
+                                                         C.c_void_p(s.cuda_stream)), "dexr_smooth_sequences_packed")
         ws.record_stream(s)
         return out, qpos, status_out
 
     def smooth_packed_sequences_vjp(self, keypoints, layout: PackedStreams, qpos, last_qpos0=None, projected0=None,
                                     grad_qpos=None, grad_robot_qpos=None, *, fixed_qpos=None, smooth_weight=None,
-                                    grad_keypoints_out=None, grad_fixed_qpos_out=None, grad_last_qpos_out=None,
-                                    status_out=None, stream=None):
+                                    accel_weight=None, grad_keypoints_out=None, grad_fixed_qpos_out=None,
+                                    grad_last_qpos_out=None, status_out=None, stream=None):
         """Backpropagation through `smooth_packed_sequences` (`dexr_smooth_sequences_packed_vjp`, one launch): the
         implicit-function VJP of the smoothed clips `qpos` [N,opt_dof] (the forward's answer) with respect to the keypoints,
         the fixed joints and the anchor.  Per-frame tensors [N,...] (keypoints, fixed_qpos, qpos, grad_qpos,
@@ -716,6 +726,7 @@ class SeqRetargeting:
         grad_last_qpos [S,opt_dof] or None when last_qpos0 is None).  The gradient is not causal: a loss on one frame
         reaches the keypoints of every frame of its stream.  A stream whose stacked Hessian is not positive definite gets
         zero gradients (STATUS_NOT_PD), one with a non-finite qpos, anchor or cotangent NaN (STATUS_NONFINITE).
+        `accel_weight` as given to the forward (`dexr_smooth_sequences_packed_accel_vjp`; None or 0: the call above).
         Allocates its workspace on the device; nothing is synchronised."""
         import torch
 
@@ -758,13 +769,20 @@ class SeqRetargeting:
         if status_out is not None:
             io.status_out = chk(status_out, (N_,), torch.int32, "status_out")
         offsets = chk(layout.offsets, (S + 1,), torch.int64, "layout.offsets")
-        nbytes = int(eng.lib.dexr_smooth_workspace_bytes(eng.handle, N_))
+        accel = 0.0 if accel_weight is None else float(accel_weight)
+        nbytes = int(eng.lib.dexr_smooth_accel_workspace_bytes(eng.handle, N_) if accel != 0.0
+                     else eng.lib.dexr_smooth_workspace_bytes(eng.handle, N_))
         ws = torch.empty((max(nbytes, 4),), dtype=torch.uint8, device=dev)
         io.workspace, io.workspace_bytes = ws.data_ptr(), nbytes
         s = stream if stream is not None else torch.cuda.current_stream(dev)
         p = opt.params(clip_init=True, lp_alpha=self.low_pass_alpha)
-        N.check(eng.lib.dexr_smooth_sequences_packed_vjp(eng.handle, C.byref(p), C.byref(io), C.c_void_p(offsets), S, N_,
-                                                         C.c_void_p(s.cuda_stream)), "dexr_smooth_sequences_packed_vjp")
+        if accel != 0.0:
+            N.check(eng.lib.dexr_smooth_sequences_packed_accel_vjp(eng.handle, C.byref(p), C.byref(io), accel,
+                                                                   C.c_void_p(offsets), S, N_, C.c_void_p(s.cuda_stream)),
+                    "dexr_smooth_sequences_packed_accel_vjp")
+        else:
+            N.check(eng.lib.dexr_smooth_sequences_packed_vjp(eng.handle, C.byref(p), C.byref(io), C.c_void_p(offsets), S,
+                                                             N_, C.c_void_p(s.cuda_stream)), "dexr_smooth_sequences_packed_vjp")
         ws.record_stream(s)
         return g_kp, g_fixed, g_last
 

@@ -522,6 +522,46 @@ int dexr_smooth_sequences_packed_vjp(const dexr_robot_t* robot, const dexr_param
                                      void* cuda_stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Offline smoothing with an acceleration penalty: dexr_smooth_sequences_packed on
+ *   F_c(X) = F(X) + c sum_{triples (t-1, t, t+1) of the stream} |x_{t+1} - 2 x_t + x_{t-1}|^2,
+ * F the smoother's objective above and c = accel_weight (finite, >= 0).  With an anchor the clipped anchor is frame -1, so the
+ * sum includes |x_1 - 2 x_0 + clip(a)|^2; a stream of fewer than two frames (three without an anchor) has no triple.  A
+ * constant-velocity trajectory costs nothing under the new term, so it damps jitter without pulling motion to a standstill
+ * the way raising w does; w = 0 with c > 0 is allowed.
+ *   The Hessian is block pentadiagonal: diagonal blocks gain 2 c m_t I (m_t the sum of the squared coefficients (1, -2, 1)
+ *   of frame t over its triples), the blocks beside them -4 c I per triple holding both frames, the blocks two away 2 c I.
+ *   It is eliminated by a banded block LDL^T along the clip: Z_t, the inverse of the Schur complement over frame t's free
+ *   variables, and the dense coupling block E_t between t and t+1 per frame; the back substitution's d_t reads d_{t+1} and
+ *   d_{t+2}.  Everything else -- the active set on the total gradient, the damping (x 0.1 / x 10), the acceptance rule, the
+ *   Gauss-Newton then more-damping restarts on a pivot <= 0, params.max_iters on accepted iterations, the DexPilot flag
+ *   walk, NONFINITE isolation per stream, status and layout -- is dexr_smooth_sequences_packed's.  A missing frame has no
+ *   data term; its value is what the smoothness terms give (with c > 0 no longer the linear interpolation).  cost_out
+ *   holds F_c at the answer.
+ *   accel_weight == 0 runs dexr_smooth_sequences_packed itself (the same bits, and its workspace size suffices).  A
+ *   non-finite or negative accel_weight returns DEXR_E_INVALID, and so does a workspace below
+ *   dexr_smooth_accel_workspace_bytes(robot, num_frames) when accel_weight > 0 (the io's workspace fields).  The call is
+ *   asynchronous on `cuda_stream`, allocates nothing and never synchronises.  All pointers are DEVICE pointers.
+ * ------------------------------------------------------------------------------------------- */
+size_t dexr_smooth_accel_workspace_bytes(const dexr_robot_t* robot, int64_t num_frames); /* >= dexr_smooth_workspace_bytes */
+int dexr_smooth_sequences_packed_accel(const dexr_robot_t* robot, const dexr_params_t* params, const dexr_smooth_t* io,
+                                       float accel_weight, const int64_t* offsets /* device [S+1] */, int64_t num_streams,
+                                       int64_t num_frames, void* cuda_stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * Backpropagation through the acceleration-penalised smoother: dexr_smooth_sequences_packed_vjp for F_c (c = accel_weight,
+ * as given to the forward; c is not differentiated).  Step 3 solves H V = G with the exact block-pentadiagonal Hessian of
+ * F_c over the free variables, by the forward's banded elimination with no damping and no fallback; step 4 is unchanged
+ * except for the anchor: grad_last_qpos = 2 w v_0 + 4 c v_0 - 2 c v_1 where clip_lo <= a <= clip_hi (0 elsewhere), the c
+ * terms only when the stream has a second frame (the triple (a, x_0, x_1)).  NOT_PD, NONFINITE, MISSING, status and layout
+ * keep their meanings.  accel_weight == 0 runs dexr_smooth_sequences_packed_vjp itself; a non-finite or negative one, or a
+ * workspace below dexr_smooth_accel_workspace_bytes(robot, num_frames) when accel_weight > 0, returns DEXR_E_INVALID.
+ * Asynchronous on `cuda_stream`, allocates nothing; all pointers are DEVICE pointers.
+ * ------------------------------------------------------------------------------------------- */
+int dexr_smooth_sequences_packed_accel_vjp(const dexr_robot_t* robot, const dexr_params_t* params, const dexr_smooth_vjp_t* io,
+                                           float accel_weight, const int64_t* offsets /* device [S+1] */,
+                                           int64_t num_streams, int64_t num_frames, void* cuda_stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Fixed-lag smoothing of live streams: every new frame re-solves the last L+1 frames of its stream jointly with the offline
  * smoother and emits the frame L ticks back.  A stream trades a fixed delay of L frames for the smoother's answer on its
  * window: no jitter from the one-sided anchor of the causal solve, dropped detections filled in from both sides.
