@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""Dry run of the GPU parity suite on the CPU: the test functions of tests/test_gpu_{parity,golden,arrow,structures,newton_step}.py are called
-unchanged while the two device entry points of the host mirror (Optimizer.retarget_batch, SeqRetargeting.retarget_sequences)
+"""Dry run of the GPU parity suite on the CPU: the test functions of tests/test_gpu_{parity,golden,arrow,structures,newton_step}.py and the
+sequences / oracle tests of tests/test_gpu_launch_chains.py (at fewer streams) are called unchanged while the two device entry points of the host mirror (Optimizer.retarget_batch, SeqRetargeting.retarget_sequences)
 are served by the HOST EMULATION of the solver source (tests/emu) -- for a chosen set of compile-time experiment switches.
 Inside the test modules `torch` is a proxy that maps every device to the CPU.  Not covered: the pinned-host entry, multi-GPU,
 anything that is specific to the kernels of dexr.cu (tile ring, alignment paths), GPU arithmetic in the last bits.
@@ -23,8 +23,9 @@ ROOT = Path(__file__).resolve().parents[2]
 for p in (ROOT, ROOT / "tests"):
     sys.path.insert(0, str(p))
 import emu_host  # noqa: E402
+import emu_seq_vjp_host  # noqa: E402
 from dex_retargeting_b200.optimizer import Optimizer  # noqa: E402
-from dex_retargeting_b200.seq_retarget import SeqRetargeting, StreamState  # noqa: E402
+from dex_retargeting_b200.seq_retarget import SequenceTape, SeqRetargeting, StreamState  # noqa: E402
 
 ARGS = sys.argv[1:]
 KEYWORD = ARGS[ARGS.index("-k") + 1] if "-k" in ARGS else None
@@ -37,6 +38,15 @@ SKIP = {"test_host_buffer_entry_matches_device_entry": "pinned-host entry (dexr_
         "test_empty_batch_is_a_no_op": "host entry",
         "test_carried_damping_through_every_entry_point": "host entries (the device part passes: 0.95 of the cold starts in the same minimum)",
         "test_mixed_launch_with_structure_cases": "mixed-robot launch (dexr_solve_frames_multi)"}
+# test_gpu_launch_chains: what the emulation has no counterpart of -- programmatic dependent launch, the tile queue, streams and
+# events, and the kernels next to the frames kernel
+_LAUNCH = "launch order on a device stream (programmatic dependent launch, tile queue, neighbouring kernels)"
+SKIP.update({name: _LAUNCH for name in (
+    "test_chain_matches_serialised_calls", "test_torch_kernel_writes_the_keypoints", "test_preprocessing_writes_the_keypoints",
+    "test_derivative_kernels_after_a_solve", "test_mixed_launch_then_single_robot", "test_two_robots_alternate_on_one_stream",
+    "test_chain_across_two_streams_joined_by_events", "test_joint_limits_changed_mid_chain")})
+# test_gpu_launch_chains at fewer streams: (module attribute, value)
+SHRINK = [("SEQ_S", 6), ("ORACLE_S", {"teleop/allegro_hand_right": 5, "teleop/leap_hand_right_dexpilot": 5})]
 
 
 class FakeEngine:
@@ -102,14 +112,30 @@ def make_stream_state(self, num_streams):
                        damping=real_torch.zeros(num_streams))
 
 
-def retarget_sequences(self, keypoints, state=None, fixed_qpos=None, out=None, status_out=None, stream=None):
+def make_sequence_tape(self, num_streams, num_steps):
+    opt = self.optimizer
+    lp = opt._objective_spec().len_proj
+    return SequenceTape(qpos=real_torch.empty((num_streams, num_steps, opt.opt_dof)),
+                        projected=(real_torch.empty((num_streams, num_steps, lp), dtype=real_torch.uint8)
+                                   if opt.retargeting_type == "DEXPILOT" else None))
+
+
+def retarget_sequences(self, keypoints, state=None, fixed_qpos=None, out=None, status_out=None, stream=None, tape=None):
     S = keypoints.shape[0]
     state = state if state is not None else self.make_stream_state(S)
     st = dict(last_qpos=_np(state.last_qpos), filter_state=_np(state.filter_state), filter_init=_np(state.filter_init),
               projected=_np(state.projected), damping=_np(state.damping))
     # DEXR_SEQ_DUO=1: the scarce-streams mode of the 16-lane solver (the library's choice for few streams unless set to 0)
-    got, status, _ = emu_host.solve_sequences(self, _np(keypoints), state=st, defines=DEFINES, use_arrow=use_arrow(),
-                                              fixed_qpos=_np(fixed_qpos), duo=os.environ.get("DEXR_SEQ_DUO") == "1")
+    duo = os.environ.get("DEXR_SEQ_DUO") == "1"
+    if tape is None:
+        got, status, _ = emu_host.solve_sequences(self, _np(keypoints), state=st, defines=DEFINES, use_arrow=use_arrow(),
+                                                  fixed_qpos=_np(fixed_qpos), duo=duo)
+    else:  # the recorded driver (dexr_solve_sequences_tape)
+        got, status, _, rec = emu_seq_vjp_host.solve_sequences_tape(self, _np(keypoints), state=st, fixed_qpos=_np(fixed_qpos),
+                                                                    use_arrow=use_arrow(), duo=duo, defines=DEFINES)
+        tape.qpos.copy_(real_torch.from_numpy(rec["qpos"]))
+        if tape.projected is not None:
+            tape.projected.copy_(real_torch.from_numpy(rec["projected"]))
     if status_out is not None:
         status_out.copy_(real_torch.from_numpy(status))
     if out is not None:
@@ -145,11 +171,14 @@ def main():
     Optimizer.retarget_batch = retarget_batch
     Optimizer.engine = lambda self: FakeEngine(self)
     SeqRetargeting.make_stream_state = make_stream_state
+    SeqRetargeting.make_sequence_tape = make_sequence_tape
     SeqRetargeting.retarget_sequences = retarget_sequences
-    import test_gpu_arrow, test_gpu_golden, test_gpu_newton_step, test_gpu_parity, test_gpu_structures  # noqa: E401
+    import test_gpu_arrow, test_gpu_golden, test_gpu_launch_chains, test_gpu_newton_step, test_gpu_parity, test_gpu_structures  # noqa: E401
 
+    for name, value in SHRINK:
+        setattr(test_gpu_launch_chains, name, value)
     failed = ran = 0
-    for mod in (test_gpu_parity, test_gpu_golden, test_gpu_arrow, test_gpu_structures, test_gpu_newton_step):
+    for mod in (test_gpu_parity, test_gpu_golden, test_gpu_arrow, test_gpu_structures, test_gpu_newton_step, test_gpu_launch_chains):
         mod.torch = TorchProxy()
         for name in [n for n in dir(mod) if n.startswith("test_")]:
             fn = getattr(mod, name)
