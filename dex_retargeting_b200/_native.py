@@ -154,6 +154,13 @@ class DexrFixedLag(C.Structure):
     ]
 
 
+class DexrFixedLagAccel(C.Structure):
+    """Mirror of `dexr_fixed_lag_accel_t`: the acceleration weight and the pre-anchor state of accelerated fixed-lag
+    streams (`dexr_fixed_lag_step_accel`)."""
+
+    _fields_ = [("accel_weight", _f), ("prev_qpos", C.c_void_p), ("has_prev", C.c_void_p)]
+
+
 class DexrFixedLagTape(C.Structure):
     """Mirror of `dexr_fixed_lag_tape_t`: what `dexr_fixed_lag_step_tape` records for the backward."""
 
@@ -204,7 +211,8 @@ EXPORTS = [
     "dexr_smooth_sequences_packed_vjp", "dexr_fixed_lag_sizeof", "dexr_fixed_lag_workspace_bytes", "dexr_fixed_lag_step",
     "dexr_fixed_lag_tape_sizeof", "dexr_fixed_lag_step_tape", "dexr_fixed_lag_vjp_sizeof",
     "dexr_fixed_lag_vjp_workspace_bytes", "dexr_fixed_lag_step_vjp", "dexr_smooth_accel_workspace_bytes",
-    "dexr_smooth_sequences_packed_accel", "dexr_smooth_sequences_packed_accel_vjp",
+    "dexr_smooth_sequences_packed_accel", "dexr_smooth_sequences_packed_accel_vjp", "dexr_fixed_lag_accel_sizeof",
+    "dexr_fixed_lag_accel_workspace_bytes", "dexr_fixed_lag_step_accel",
 ]
 
 _LIB = None
@@ -363,6 +371,17 @@ def load():
                                                 C.c_int64, C.c_void_p]
     elif not os.environ.get("DEXR_LIBRARY"):
         raise DexrError(f"{path} does not export dexr_fixed_lag_vjp_sizeof: rebuild it "
+                        "(python -m dex_retargeting_b200.build --force)")
+    if hasattr(lib, "dexr_fixed_lag_accel_sizeof"):
+        lib.dexr_fixed_lag_accel_sizeof.restype = C.c_size_t
+        if lib.dexr_fixed_lag_accel_sizeof() != C.sizeof(DexrFixedLagAccel):
+            raise DexrError("dexr_fixed_lag_accel_t layout mismatch between library and binding (stale DEXR_LIBRARY?)")
+        lib.dexr_fixed_lag_accel_workspace_bytes.argtypes = [C.c_void_p, C.c_int64, C.c_int32]
+        lib.dexr_fixed_lag_accel_workspace_bytes.restype = C.c_size_t
+        lib.dexr_fixed_lag_step_accel.argtypes = [C.c_void_p, C.POINTER(DexrParams), C.POINTER(DexrFixedLag),
+                                                  C.POINTER(DexrFixedLagAccel), C.c_int64, C.c_int64, C.c_void_p]
+    elif not os.environ.get("DEXR_LIBRARY"):
+        raise DexrError(f"{path} does not export dexr_fixed_lag_accel_sizeof: rebuild it "
                         "(python -m dex_retargeting_b200.build --force)")
     # (an older A/B library named by DEXR_LIBRARY reads a prefix of the buffer structs -- fields are only ever appended -- so
     # the single-robot entry points still work with it; dexr_solve_frames_multi, whose groups embed the struct, does not)

@@ -754,10 +754,12 @@ struct FixedLagArgs {
   int pos_off;  // shared memory: each warp's loop state, 2 long longs
 };
 
-// The body of dexr_fixed_lag_kernel and dexr_fixed_lag_tape_kernel; REC (dexr_fixed_lag_step_tape): fixed_lag_tick's
-// recording into `tape`.
-template <int G, bool REC>
-__device__ __forceinline__ void fixed_lag_kernel_body(const FixedLagArgs& a, const dexr_fixed_lag_tape_t& tape) {
+// The body of dexr_fixed_lag_kernel, dexr_fixed_lag_tape_kernel and dexr_fixed_lag_accel_kernel; REC
+// (dexr_fixed_lag_step_tape): fixed_lag_tick's recording into `tape`; ACC (dexr_fixed_lag_step_accel): the ticks and the
+// flush of acceleration-penalised streams with the pre-anchor state `acc`.
+template <int G, bool REC, bool ACC = false>
+__device__ __forceinline__ void fixed_lag_kernel_body(const FixedLagArgs& a, const dexr_fixed_lag_tape_t& tape,
+                                                      const dexr_fixed_lag_accel_t* acc = nullptr) {
   load_shared_table(*reinterpret_cast<SharedTable*>(dsmem), a.table);
   __syncthreads();
   constexpr int GPW = 32 / G;
@@ -779,7 +781,7 @@ __device__ __forceinline__ void fixed_lag_kernel_body(const FixedLagArgs& a, con
     }
     __syncwarp();
     while (pos[0] < a.S) {
-      fixed_lag_tick<G, REC>(sv, a.io, a.dm, a.prm, a.wstatus, a.K, pos, lane < G, tape.qpos, tape.projected);
+      fixed_lag_tick<G, REC, ACC>(sv, a.io, a.dm, a.prm, a.wstatus, a.K, pos, lane < G, tape.qpos, tape.projected, acc);
       if (lane == 0) {
         if (pos[1] + 1 < a.K) {
           pos[1] = pos[1] + 1;
@@ -792,7 +794,8 @@ __device__ __forceinline__ void fixed_lag_kernel_body(const FixedLagArgs& a, con
     }
   }
   if (a.flush)
-    for (long long s = first; s < a.S; s += (long long)gridDim.x * kEvalWarps) fixed_lag_flush(sv, a.io, a.dm, a.prm, s, lane < G);
+    for (long long s = first; s < a.S; s += (long long)gridDim.x * kEvalWarps)
+      fixed_lag_flush<G, ACC>(sv, a.io, a.dm, a.prm, s, lane < G, acc);
 }
 
 template <int G>
@@ -805,6 +808,14 @@ template <int G>
 __global__ void __launch_bounds__(kEvalWarps * 32, G == 16 ? 2 : 1) dexr_fixed_lag_tape_kernel(const FixedLagArgs a,
                                                                                                const dexr_fixed_lag_tape_t tape) {
   fixed_lag_kernel_body<G, true>(a, tape);
+}
+
+// dexr_fixed_lag_step_accel: dexr_fixed_lag_kernel with the acceleration-penalised window solve and the pre-anchor state
+// (its own kernel, so that the velocity-only one keeps its code; the smoother's workspace per frame is SmoothAccWs<G>).
+template <int G>
+__global__ void __launch_bounds__(kEvalWarps * 32, G == 16 ? 2 : 1) dexr_fixed_lag_accel_kernel(
+    const FixedLagArgs a, const __grid_constant__ dexr_fixed_lag_accel_t acc) {
+  fixed_lag_kernel_body<G, false, true>(a, dexr_fixed_lag_tape_t{nullptr, nullptr}, &acc);
 }
 
 // backpropagation through fixed-lag smoothing: dexr_smooth_vjp_kernel's launch shape, the streams dealt as
@@ -2193,10 +2204,13 @@ extern "C" int dexr_smooth_sequences_packed_accel_vjp(const dexr_robot_t* robot,
                                    : launch_smooth_accel_vjp<32>(r, params, io, accel_weight, pk, stream);
 }
 
-// dexr_fixed_lag_step: launch_smooth's CTA and occupancy rule.
+// dexr_fixed_lag_step: launch_smooth's CTA and occupancy rule.  `tape`: dexr_fixed_lag_step_tape's recording; `acc`:
+// dexr_fixed_lag_step_accel's pre-anchor state (dexr_fixed_lag_accel_kernel, its own occupancy, the status words after the
+// accel smoother's workspace).
 template <int G>
 static int launch_fixed_lag(dexr_robot* r, const dexr_params_t* prm, const dexr_fixed_lag_t* io, long long S, int K,
-                            cudaStream_t stream, const dexr_fixed_lag_tape_t* tape = nullptr) {
+                            cudaStream_t stream, const dexr_fixed_lag_tape_t* tape = nullptr,
+                            const dexr_fixed_lag_accel_t* acc = nullptr) {
   FixedLagArgs a{};
   a.table = r->table_dev;
   a.prm = *prm;
@@ -2205,7 +2219,7 @@ static int launch_fixed_lag(dexr_robot* r, const dexr_params_t* prm, const dexr_
   a.S = S;
   a.K = K;
   a.flush = io->flush_count_out != nullptr;
-  a.wstatus = fixed_lag_status_words<G>(*io, S);
+  a.wstatus = acc ? fixed_lag_status_words<G, true>(*io, S) : fixed_lag_status_words<G>(*io, S);
   a.dm = make_dims(r->host);
   a.scratch_off = round_up((int)sizeof(SharedTable), 16);
   constexpr int GPW = 32 / G;
@@ -2213,12 +2227,15 @@ static int launch_fixed_lag(dexr_robot* r, const dexr_params_t* prm, const dexr_
   const int smem = a.pos_off + kEvalWarps * 2 * (int)sizeof(long long);
   auto kern = dexr_fixed_lag_kernel<G>;
   auto kern_tape = dexr_fixed_lag_tape_kernel<G>;
+  auto kern_acc = dexr_fixed_lag_accel_kernel<G>;
   CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
   if (tape) CUDA_TRY(cudaFuncSetAttribute(kern_tape, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  if (acc) CUDA_TRY(cudaFuncSetAttribute(kern_acc, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
   int per_sm = 1;
-  if (int e = eval_ctas_per_sm(kern, smem, &per_sm)) return e;
+  if (int e = acc ? eval_ctas_per_sm(kern_acc, smem, &per_sm) : eval_ctas_per_sm(kern, smem, &per_sm)) return e;
   const int grid = (int)std::min<long long>(S, (long long)r->num_sms * per_sm);
-  if (tape) kern_tape<<<grid, kEvalWarps * 32, smem, stream>>>(a, *tape);
+  if (acc) kern_acc<<<grid, kEvalWarps * 32, smem, stream>>>(a, *acc);
+  else if (tape) kern_tape<<<grid, kEvalWarps * 32, smem, stream>>>(a, *tape);
   else kern<<<grid, kEvalWarps * 32, smem, stream>>>(a);
   CUDA_TRY(cudaGetLastError());
   {
@@ -2246,6 +2263,28 @@ extern "C" int dexr_fixed_lag_step(const dexr_robot_t* robot, const dexr_params_
   cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
   return eval_lanes(r->host) == 16 ? launch_fixed_lag<16>(r, params, io, num_streams, (int)num_ticks, stream)
                                    : launch_fixed_lag<32>(r, params, io, num_streams, (int)num_ticks, stream);
+}
+
+extern "C" size_t dexr_fixed_lag_accel_sizeof(void) { return sizeof(dexr_fixed_lag_accel_t); }
+
+extern "C" size_t dexr_fixed_lag_accel_workspace_bytes(const dexr_robot_t* robot, int64_t num_streams, int32_t lag) {
+  return robot ? fixed_lag_accel_workspace_bytes(robot->host, num_streams, lag) : 0;
+}
+
+extern "C" int dexr_fixed_lag_step_accel(const dexr_robot_t* robot, const dexr_params_t* params, const dexr_fixed_lag_t* io,
+                                         const dexr_fixed_lag_accel_t* acc, int64_t num_streams, int64_t num_ticks,
+                                         void* cuda_stream) {
+  if (!robot || !params || !io || !acc) return fail(DEXR_E_INVALID, "dexr_fixed_lag_step_accel: null argument");
+  if (const char* msg = fixed_lag_io_error(robot->host, *io, *params, num_streams, num_ticks))
+    return fail(DEXR_E_INVALID, "%s", msg);
+  if (const char* msg = fixed_lag_accel_error(robot->host, *io, *acc, num_streams)) return fail(DEXR_E_INVALID, "%s", msg);
+  if (int e = check_params(params)) return e;
+  if (num_streams == 0 || (num_ticks == 0 && !io->flush_count_out)) return 0;
+  DEVICE_SCOPE(robot->device);
+  dexr_robot* r = const_cast<dexr_robot*>(robot);
+  cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
+  return eval_lanes(r->host) == 16 ? launch_fixed_lag<16>(r, params, io, num_streams, (int)num_ticks, stream, nullptr, acc)
+                                   : launch_fixed_lag<32>(r, params, io, num_streams, (int)num_ticks, stream, nullptr, acc);
 }
 
 extern "C" size_t dexr_fixed_lag_tape_sizeof(void) { return sizeof(dexr_fixed_lag_tape_t); }

@@ -2798,6 +2798,27 @@ struct AccTerms {
   }
 };
 
+// The pre-anchor of a fixed-lag window solve with the acceleration penalty (smooth_packed_stream<G, true, true>,
+// dexr_fixed_lag_step_accel, DESIGN.md 3.17).  Its state travels in io.cost_out, which a window solve leaves NULL (it
+// writes no cost), as c travels in io.smooth_weight: a parameter of its own changes the code of the instantiations without
+// it.  Read at each use rather than held in registers across the solve.
+__device__ __forceinline__ const dexr_fixed_lag_accel_t* pre_anchor_state(const dexr_smooth_t& io) {
+  return reinterpret_cast<const dexr_fixed_lag_accel_t*>(io.cost_out);
+}
+// Whether stream s has a pre-anchor (has_prev[s] non-zero; group-uniform).
+__device__ __forceinline__ bool pre_anchor_on(const dexr_smooth_t& io, long long s, bool has) {
+  return has && pre_anchor_state(io)->has_prev[s] != 0;
+}
+// The residual x - 2 clip(a) + clip(p) of the triple (p, a, x_0) on this var lane (`a`: its clip(a)); the stream has a
+// pre-anchor.
+template <int G>
+__device__ __forceinline__ float pre_anchor_res(const Solver<G, 0>& sv, const dexr_smooth_t& io, long long s, int n, float a,
+                                                float x) {
+  const SharedTable& st = Solver<G, 0>::ST();
+  const float p = fminf(fmaxf(pre_anchor_state(io)->prev_qpos[s * n + sv.var], st.clip_lo[sv.l]), st.clip_hi[sv.l]);
+  return x - 2.f * a + p;
+}
+
 // The banded block elimination's share of frame t (ACC), between fold_free_block and factor_rows: with the dense coupling
 // E_{t-1} between frames t-1 and t and P = Z_{t-1} E_{t-1} (column per lane, in the kH area),
 //   S_t = D_t - E_{t-1}^T P - c2^2 Z_{t-2},   y_t = y - P^T y_{t-1} - c2 Z_{t-2} y_{t-2},   E_t = b I - c1 P^T
@@ -2872,9 +2893,14 @@ __device__ __forceinline__ float accel_back_rhs(const float* wt, int l, int dof,
 // block Thomas, SmoothAccWs<G>::kFloats per frame; everything else as above.  c is io.smooth_weight: the launch has moved w
 // into sv.prm.norm_delta, and c travels in the io rather than in a parameter of its own, which would change the code of the
 // velocity-only instantiation.
-template <int G, bool ACC = false>
+// PRE (with ACC; dexr_fixed_lag_step_accel, DESIGN.md 3.17): stream s with has_prev[s] non-zero in the pre-anchor state
+// (pre_anchor_state: io.cost_out, so no cost is written) adds the triple (clip(prev_qpos[s]), clip(a), x_0):
+// c |x_0 - 2 clip(a) + clip(p)|^2 joins F_0, x_0's gradient and x_0's diagonal block (+2c); nothing off the diagonal
+// changes.  A non-finite prev_qpos there is a non-finite start.
+template <int G, bool ACC = false, bool PRE = false>
 __device__ __forceinline__ void smooth_packed_stream(Solver<G, 0>& sv, const dexr_smooth_t& io, const Dims& dm,
                                                      const dexr_params_t& prm, const PackedStream& ps, bool owner, float* ws) {
+  static_assert(ACC || !PRE, "the pre-anchor is a triple of the acceleration penalty");
   using W = typename SmoothWsOf<G, ACC>::type;
   constexpr int NP = G;
   const SharedTable& st = Solver<G, 0>::ST();
@@ -2900,6 +2926,8 @@ __device__ __forceinline__ void smooth_packed_stream(Solver<G, 0>& sv, const dex
     const float ar = io.last_qpos[sc * n + sv.var];
     nonfinite = !isfinite(ar);
     a = fminf(fmaxf(ar, st.clip_lo[l]), st.clip_hi[l]);
+    if constexpr (PRE)
+      if (pre_anchor_on(io, sc, has)) nonfinite = nonfinite || !isfinite(pre_anchor_state(io)->prev_qpos[sc * n + sv.var]);
   }
   for (int t = 0; t < len; ++t) {
     float x = 0.f;
@@ -2938,7 +2966,12 @@ __device__ __forceinline__ void smooth_packed_stream(Solver<G, 0>& sv, const dex
       const float v = smooth_eval(sv, io, dm, fr, x, xp, has_prev, missing, live);
       if constexpr (ACC) {  // with the triples' share of F_t
         const float xp2 = (live && t > 1) ? wt[W::kX + cur * G + l - 2 * W::kFloats] : a;
-        const float va = isvar ? v + AccTerms(t, len, anchor).cost(io.smooth_weight, xp2, xp, x) : v;
+        float va = isvar ? v + AccTerms(t, len, anchor).cost(io.smooth_weight, xp2, xp, x) : v;
+        if constexpr (PRE)
+          if (t == 0 && isvar && pre_anchor_on(io, sc, has)) {  // the triple (p, a, x_0)
+            const float r = pre_anchor_res(sv, io, sc, n, a, x);
+            va += io.smooth_weight * r * r;
+          }
         if (live) {
           wt[W::kV + l] = va;
           fsum += va;
@@ -2959,6 +2992,9 @@ __device__ __forceinline__ void smooth_packed_stream(Solver<G, 0>& sv, const dex
         const float xp2 = (live && t > 1) ? wt[W::kX + cur * G + l - 2 * W::kFloats] : a;
         const float xn2 = (live && at.left) ? wt[W::kX + cur * G + l + 2 * W::kFloats] : 0.f;
         if (isvar) g += at.grad(io.smooth_weight, xp2, xp, x, xn, xn2);
+        if constexpr (PRE)
+          if (t == 0 && isvar && pre_anchor_on(io, sc, has))  // the triple (p, a, x_0)
+            g += 2.f * io.smooth_weight * pre_anchor_res(sv, io, sc, n, a, x);
       }
       const bool at_bound = isvar && ((x <= sv.lo && g > -kGradNoise) || (x >= sv.hi && g < kGradNoise));
       const bool free_ = live && isvar && !at_bound;
@@ -2969,6 +3005,9 @@ __device__ __forceinline__ void smooth_packed_stream(Solver<G, 0>& sv, const dex
                                                       fmaf(w2, (float)((has_prev ? 1 : 0) + (has_next ? 1 : 0)), mu)));
       else
         fold_free_block(sv, dm, A, free_, fmask, fmaf(w2, (float)((has_prev ? 1 : 0) + (has_next ? 1 : 0)), mu));
+      if constexpr (PRE)
+        if (t == 0 && free_ && pre_anchor_on(io, sc, has))  // the triple (p, a, x_0): +2c on x_0's diagonal (row l: this lane's)
+          A[l * (NP + 1) + l] += 2.f * io.smooth_weight;
       float y = free_ ? -g : 0.f;
       if constexpr (ACC)
         y = accel_eliminate<G, W>(sv, dof, A, wt, t, live, free_, fmask, y, yprev,
@@ -3055,7 +3094,12 @@ __device__ __forceinline__ void smooth_packed_stream(Solver<G, 0>& sv, const dex
       const float v = smooth_eval(sv, io, dm, fr, x, xp, t > 0 || anchor, missing, live);
       if constexpr (ACC) {  // with the triples' share of F_t
         const float xp2 = (live && t > 1) ? wt[W::kX + (cur ^ 1) * G + l - 2 * W::kFloats] : a;
-        const float va = isvar ? v + AccTerms(t, len, anchor).cost(io.smooth_weight, xp2, xp, x) : v;
+        float va = isvar ? v + AccTerms(t, len, anchor).cost(io.smooth_weight, xp2, xp, x) : v;
+        if constexpr (PRE)
+          if (t == 0 && isvar && pre_anchor_on(io, sc, has)) {  // the triple (p, a, x_0)
+            const float r = pre_anchor_res(sv, io, sc, n, a, x);
+            va += io.smooth_weight * r * r;
+          }
         if (live) {
           dsum += va - wt[W::kV + l];
           fnew += va;
@@ -3102,7 +3146,8 @@ __device__ __forceinline__ void smooth_packed_stream(Solver<G, 0>& sv, const dex
       if (io.status_out && l == 0) io.status_out[fr] = base_status | (missing ? DEXR_STATUS_MISSING : 0);
     }
   }
-  if (has && io.cost_out && l == 0) io.cost_out[sc] = nonfinite ? __int_as_float(0x7fc00000) : F;
+  if constexpr (!PRE)
+    if (has && io.cost_out && l == 0) io.cost_out[sc] = nonfinite ? __int_as_float(0x7fc00000) : F;
   __syncwarp();
 }
 
@@ -3363,10 +3408,19 @@ inline size_t fixed_lag_workspace_bytes(const dexr_table_t& t, long long S, long
   return smooth_workspace_bytes(t, frames) + (size_t)frames * sizeof(int32_t);
 }
 
-// Where the status words of a G-lane call's workspace start.
-template <int G>
+// Bytes of workspace an acceleration-penalised call needs (dexr_fixed_lag_accel_workspace_bytes): the accel smoother's for
+// S (L+1) frames, then the S (L+1) status words.
+inline size_t fixed_lag_accel_workspace_bytes(const dexr_table_t& t, long long S, long long lag) {
+  if (S <= 0 || lag < 0 || lag > DEXR_FIXED_LAG_MAX) return 0;
+  const long long frames = S * (lag + 1);
+  return smooth_accel_workspace_bytes(t, frames) + (size_t)frames * sizeof(int32_t);
+}
+
+// Where the status words of a G-lane call's workspace start (ACC: after the accel smoother's frames).
+template <int G, bool ACC = false>
 inline int32_t* fixed_lag_status_words(const dexr_fixed_lag_t& io, long long S) {
-  return reinterpret_cast<int32_t*>(static_cast<float*>(io.workspace) + S * (io.lag + 1) * SmoothWs<G>::kFloats);
+  return reinterpret_cast<int32_t*>(static_cast<float*>(io.workspace) +
+                                    S * (io.lag + 1) * SmoothWsOf<G, ACC>::type::kFloats);
 }
 
 // The argument checks of dexr_fixed_lag_step: nullptr, or what is wrong.  Host code shared by the library and the host
@@ -3387,6 +3441,17 @@ inline const char* fixed_lag_io_error(const dexr_table_t& t, const dexr_fixed_la
     return "smooth_weight must be finite (< 0: params.norm_delta)";
   if (S > 0 && (!io.workspace || io.workspace_bytes < fixed_lag_workspace_bytes(t, S, io.lag)))
     return "workspace smaller than dexr_fixed_lag_workspace_bytes(robot, num_streams, lag)";
+  return nullptr;
+}
+
+// The extra argument checks of dexr_fixed_lag_step_accel (after fixed_lag_io_error): nullptr, or what is wrong.
+inline const char* fixed_lag_accel_error(const dexr_table_t& t, const dexr_fixed_lag_t& io, const dexr_fixed_lag_accel_t& acc,
+                                         long long S) {
+  if (!(acc.accel_weight > 0.f && acc.accel_weight <= 3.0e38f))
+    return "accel_weight must be finite and > 0 (c = 0 streams use dexr_fixed_lag_step)";
+  if (S > 0 && (!acc.prev_qpos || !acc.has_prev)) return "prev_qpos and has_prev are required";
+  if (S > 0 && io.workspace_bytes < fixed_lag_accel_workspace_bytes(t, S, io.lag))
+    return "workspace smaller than dexr_fixed_lag_accel_workspace_bytes(robot, num_streams, lag)";
   return nullptr;
 }
 
@@ -3442,6 +3507,16 @@ __device__ __forceinline__ float fixed_lag_emit(Solver<G, 0>& sv, const dexr_fix
   return x;
 }
 
+// Before a commit of an acceleration-penalised stream s: the anchor (raw) becomes prev_qpos and has_prev is set (each var
+// lane moves its own entry; the caller's __syncwarp orders lane 0's has_prev for the next solve).
+template <int G>
+__device__ __forceinline__ void fixed_lag_commit_pre(const Solver<G, 0>& sv, const dexr_fixed_lag_t& io,
+                                                     const dexr_fixed_lag_accel_t& acc, const Dims& dm, long long s,
+                                                     bool owner) {
+  if (owner && sv.var >= 0) acc.prev_qpos[s * dm.n_var + sv.var] = io.last_qpos[s * dm.n_var + sv.var];
+  if (owner && sv.l == 0) acc.has_prev[s] = 1;
+}
+
 // One tick of dexr_fixed_lag_step: tick pos[1] of stream pos[0] (< S).  `pos` is the caller's loop state, read again after
 // the window solve: no index of the driver stays in a register across the smoother, which uses every register the 16-lane
 // kernel has (128); window_len is stored before the solve (the count includes the incoming frame from the append on) and
@@ -3450,12 +3525,14 @@ __device__ __forceinline__ float fixed_lag_emit(Solver<G, 0>& sv, const dexr_fix
 // window_len too).  `wstatus`: the status words after the smoother's part of the workspace.  Between a lane's global
 // writes and another lane's reads, __syncwarp.  REC (dexr_fixed_lag_step_tape): after the solve, the window minimiser goes
 // to tape_qpos [S,K,L+1,n_var] and the committed flags the solve started from to tape_projected [S,K,len_proj] (nullptr:
-// none).
-template <int G, bool REC = false>
+// none).  ACC (dexr_fixed_lag_step_accel): the window solve is smooth_packed_stream<G, true, true> with c =
+// acc->accel_weight and the stream's pre-anchor; a commit first moves the old anchor to prev_qpos and sets has_prev.
+template <int G, bool REC = false, bool ACC = false>
 __device__ __forceinline__ void fixed_lag_tick(Solver<G, 0>& sv, const dexr_fixed_lag_t& io, const Dims& dm,
                                                const dexr_params_t& prm, int32_t* wstatus, int K,
                                                const volatile long long* pos, bool owner, float* tape_qpos = nullptr,
-                                               uint8_t* tape_projected = nullptr) {
+                                               uint8_t* tape_projected = nullptr,
+                                               const dexr_fixed_lag_accel_t* acc = nullptr) {
   constexpr int KP = 3 * DEXR_NUM_KEYPOINTS;
   const int l = sv.l, n = dm.n_var, nf = dm.n_fixed, L = io.lag, W1 = L + 1;
   const bool isvar = sv.var >= 0;
@@ -3485,7 +3562,14 @@ __device__ __forceinline__ void fixed_lag_tick(Solver<G, 0>& sv, const dexr_fixe
     sio.qpos_out = io.window_qpos;
     sio.status_out = wstatus;
     sio.workspace = io.workspace;
-    smooth_packed_stream(sv, sio, dm, prm, PackedStream{s, s * W1, io.window_len[s]}, owner, static_cast<float*>(io.workspace));
+    if constexpr (ACC) {
+      sio.smooth_weight = acc->accel_weight;  // (w is in sv.prm.norm_delta)
+      sio.cost_out = reinterpret_cast<float*>(const_cast<dexr_fixed_lag_accel_t*>(acc));  // (pre_anchor_state)
+      smooth_packed_stream<G, true, true>(sv, sio, dm, prm, PackedStream{s, s * W1, io.window_len[s]}, owner,
+                                          static_cast<float*>(io.workspace));
+    } else {
+      smooth_packed_stream(sv, sio, dm, prm, PackedStream{s, s * W1, io.window_len[s]}, owner, static_cast<float*>(io.workspace));
+    }
   }
   if constexpr (REC) {  // (each var lane copies the entries it wrote itself)
     const long long s = pos[0], t = s * K + pos[1];
@@ -3500,6 +3584,7 @@ __device__ __forceinline__ void fixed_lag_tick(Solver<G, 0>& sv, const dexr_fixe
   const float x = fixed_lag_emit(sv, io, dm, s, 0, full, owner, io.qpos_out, io.robot_qpos_out, fin);
   if (owner && l == 0 && io.status_out) io.status_out[fin] = full ? wstatus[w0] : DEXR_STATUS_PENDING;
   if (full) {
+    if constexpr (ACC) fixed_lag_commit_pre(sv, io, *acc, dm, s, owner);
     if (owner && isvar) io.last_qpos[s * n + sv.var] = x;
     fixed_lag_advance_flags(sv, dm, prm, io.window_keypoints + w0 * KP,
                             dm.len_proj > 0 ? io.projected + s * dm.len_proj : nullptr, owner);
@@ -3517,10 +3602,12 @@ __device__ __forceinline__ void fixed_lag_tick(Solver<G, 0>& sv, const dexr_fixe
 }
 
 // The flush of stream s (< S) of dexr_fixed_lag_step: the held frames as the last solve left them, in order; the last becomes
-// the anchor, the flags advance through them and the window empties.  `owner` as in fixed_lag_tick.
-template <int G>
+// the anchor, the flags advance through them and the window empties.  `owner` as in fixed_lag_tick.  ACC: each commit moves
+// the anchor to the pre-anchor first (fixed_lag_commit_pre), as a tick's does.
+template <int G, bool ACC = false>
 __device__ __forceinline__ void fixed_lag_flush(Solver<G, 0>& sv, const dexr_fixed_lag_t& io, const Dims& dm,
-                                                const dexr_params_t& prm, long long s, bool owner) {
+                                                const dexr_params_t& prm, long long s, bool owner,
+                                                const dexr_fixed_lag_accel_t* acc = nullptr) {
   const int l = sv.l, L = io.lag, W1 = L + 1;
   const int h0 = io.window_len[s];
   const int h = h0 < 0 ? 0 : (h0 > L ? L : h0);
@@ -3529,6 +3616,7 @@ __device__ __forceinline__ void fixed_lag_flush(Solver<G, 0>& sv, const dexr_fix
     const bool held = j < h;
     const float x = fixed_lag_emit(sv, io, dm, s, j, held, owner, io.flush_qpos_out, io.flush_robot_qpos_out, s * L + j);
     if (held) {
+      if constexpr (ACC) fixed_lag_commit_pre(sv, io, *acc, dm, s, owner);
       if (owner && sv.var >= 0) io.last_qpos[s * dm.n_var + sv.var] = x;
       fixed_lag_advance_flags(sv, dm, prm, io.window_keypoints + (s * W1 + j) * (3 * DEXR_NUM_KEYPOINTS), flags, owner);
     }

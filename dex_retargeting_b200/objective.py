@@ -308,9 +308,11 @@ def differentiable_retarget_fixed_lag(seq, keypoints, state, fixed_qpos=None, *,
     is not modified, and the returned FixedLagState's last_qpos and window tensors carry the graph, so chunks of a live
     stream backpropagate across call boundaries (detach the state for truncated backpropagation).  backward() is one
     `retarget_fixed_lag_vjp` launch: each emitting window's smoother VJP, the anchor chain through the committed frames.
-    PENDING rows (NaN) get no gradient.  The DexPilot flags and `smooth_weight` are not differentiated."""
-    from .seq_retarget import FixedLagState
+    PENDING rows (NaN) get no gradient.  The DexPilot flags and `smooth_weight` are not differentiated.  A state with an
+    acceleration penalty is refused (ValueError): there is no backward through it yet."""
+    from .seq_retarget import FixedLagState, _refuse_accel_backward
 
+    _refuse_accel_backward(state, "differentiable_retarget_fixed_lag")
     if isinstance(smooth_weight, torch.Tensor):
         if smooth_weight.requires_grad:
             raise ValueError("smooth_weight requires grad, but fixed-lag smoothing is not differentiated in it: detach it")
@@ -348,9 +350,11 @@ class _DifferentiableFlushFixedLag(torch.autograd.Function):
 def differentiable_flush_fixed_lag(seq, state):
     """(robot_qpos [S,L,dof], qpos [S,L,opt_dof], count [S], new_state) = `seq.flush_fixed_lag(state)`, differentiable in
     the state's `last_qpos` and window tensors (the flushed rows are its held slots of window_qpos).  `state` is not
-    modified; the returned state carries the graph as `differentiable_retarget_fixed_lag`'s does."""
-    from .seq_retarget import FixedLagState
+    modified; the returned state carries the graph as `differentiable_retarget_fixed_lag`'s does.  A state with an
+    acceleration penalty is refused (ValueError), as there."""
+    from .seq_retarget import FixedLagState, _refuse_accel_backward
 
+    _refuse_accel_backward(state, "differentiable_flush_fixed_lag")
     cfg = dict(state=state)
     rq, q, count, last, wkp, wfix, wq = _DifferentiableFlushFixedLag.apply(
         state.last_qpos, state.window_keypoints, state.window_fixed_qpos, state.window_qpos, seq, cfg)

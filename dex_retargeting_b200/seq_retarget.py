@@ -16,7 +16,7 @@ end (`PackedStreams`, the cu_seqlens layout): recorded clips of any length in on
 `smooth_packed_sequences()` solves every frame of each packed clip jointly (`dexr_smooth_sequences_packed`): the offline
 trajectory, with no lag and with dropped frames filled in.  `retarget_fixed_lag()` brings it to live streams
 (`dexr_fixed_lag_step`, `FixedLagState`): each new frame re-solves the last L+1 frames jointly and emits the frame L ticks
-back.
+back; a state made with `accel_weight` also penalises acceleration there (`dexr_fixed_lag_step_accel`).
 """
 from __future__ import annotations
 
@@ -88,23 +88,37 @@ class FixedLagState:
     window_fixed_qpos: Optional["torch.Tensor"]  # [S, L+1, n_fixed] float32, or None without fixed joints
     window_qpos: "torch.Tensor"        # [S, L+1, opt_dof] float32
     window_len: "torch.Tensor"         # [S] int32, frames held (0..L)
+    # the acceleration penalty c (`dexr_fixed_lag_step_accel`), fixed for the life of the state like the lag; 0: none, and
+    # the two fields after it are None
+    accel_weight: float = 0.0
+    prev_qpos: Optional["torch.Tensor"] = None  # [S, opt_dof] float32, the frame committed before last_qpos (raw)
+    has_prev: Optional["torch.Tensor"] = None   # [S] int32, 0 fresh, 1 after the first commit
 
-    _FIELDS = ("last_qpos", "projected", "window_keypoints", "window_fixed_qpos", "window_qpos", "window_len")
+    _FIELDS = ("last_qpos", "projected", "window_keypoints", "window_fixed_qpos", "window_qpos", "window_len", "prev_qpos",
+               "has_prev")
 
     def state_dict(self) -> dict:
-        """Host copies of every tensor (None stays None) and the lag: a run resumed from it continues bit-identically."""
-        d = {k: (None if getattr(self, k) is None else getattr(self, k).detach().cpu().clone()) for k in self._FIELDS}
+        """Host copies of every tensor (None stays None) and the lag: a run resumed from it continues bit-identically.  An
+        accelerated state also holds accel_weight, prev_qpos and has_prev; a c = 0 state has none of these keys."""
+        keys = self._FIELDS if self.accel_weight else self._FIELDS[:-2]
+        d = {k: (None if getattr(self, k) is None else getattr(self, k).detach().cpu().clone()) for k in keys}
         d["lag"] = int(self.lag)
+        if self.accel_weight:
+            d["accel_weight"] = float(self.accel_weight)
         return d
 
     @classmethod
     def from_state_dict(cls, state: dict, device=None) -> "FixedLagState":
-        """Inverse of `state_dict`: copies of its tensors on `device`."""
+        """Inverse of `state_dict`: copies of its tensors on `device`.  A checkpoint without accel_weight is a c = 0 state."""
         import torch
 
-        missing = [k for k in ("lag", "last_qpos", "window_keypoints", "window_qpos", "window_len") if state.get(k) is None]
+        accel = float(state.get("accel_weight") or 0.0)
+        required = ("lag", "last_qpos", "window_keypoints", "window_qpos", "window_len")
+        missing = [k for k in required + (("prev_qpos", "has_prev") if accel else ()) if state.get(k) is None]
         if missing:
             raise ValueError(f"fixed-lag state checkpoint lacks {missing}")
+        if not accel and (state.get("prev_qpos") is not None or state.get("has_prev") is not None):
+            raise ValueError("fixed-lag state checkpoint: prev_qpos / has_prev without accel_weight")
         S, lag = int(state["last_qpos"].shape[0]), int(state["lag"])
         for k in cls._FIELDS[1:]:
             t = state.get(k)
@@ -118,7 +132,15 @@ class FixedLagState:
         def put(t):  # (a copy: the restored state never aliases the checkpoint)
             return None if t is None else torch.as_tensor(t).to(device if device is not None else t.device, copy=True).contiguous()
 
-        return cls(lag=lag, **{k: put(state.get(k)) for k in cls._FIELDS})
+        return cls(lag=lag, accel_weight=accel, **{k: put(state.get(k)) for k in cls._FIELDS})
+
+
+def _refuse_accel_backward(state: FixedLagState, what: str, taped: bool = True):
+    """The backward through accelerated fixed-lag streams (a window tape and VJP with two anchor cotangents) does not exist
+    yet: refuse rather than differentiate the velocity-only problem."""
+    if taped and state.accel_weight:
+        raise ValueError(f"{what}: there is no backward through fixed-lag streams with an acceleration penalty "
+                         f"(accel_weight = {state.accel_weight}); only the forward and the flush run on them")
 
 
 @dataclass
@@ -786,14 +808,20 @@ class SeqRetargeting:
         ws.record_stream(s)
         return g_kp, g_fixed, g_last
 
-    def make_fixed_lag_state(self, num_streams: int, lag: int) -> FixedLagState:
+    def make_fixed_lag_state(self, num_streams: int, lag: int, accel_weight: Optional[float] = None) -> FixedLagState:
         """Initial state of S fresh live streams smoothed with lag L (`retarget_fixed_lag`): the anchor at the mid-range warm
-        start (as `make_stream_state`; `warm_start_batch` applies to `last_qpos`), no DexPilot projection, an empty window."""
+        start (as `make_stream_state`; `warm_start_batch` applies to `last_qpos`), no DexPilot projection, an empty window.
+        `accel_weight` c > 0: each window solve also penalises c |x_{t+1} - 2 x_t + x_{t-1}|^2, the frame committed before
+        the anchor counting as frame -2 (`dexr_fixed_lag_step_accel`); the state then carries prev_qpos and has_prev.  c
+        is fixed for the life of the state; None or 0: no acceleration penalty."""
         import torch
 
         lag = int(lag)
         if not 0 <= lag <= N.FIXED_LAG_MAX:
             raise ValueError(f"lag must be in 0..{N.FIXED_LAG_MAX}, got {lag}")
+        accel = 0.0 if accel_weight is None else float(accel_weight)
+        if not (accel == 0.0 or 0.0 < accel <= 3.0e38):
+            raise ValueError(f"accel_weight must be finite and >= 0, got {accel_weight}")
         opt = self.optimizer
         base = self.make_stream_state(num_streams)
         dev = base.last_qpos.device
@@ -803,7 +831,9 @@ class SeqRetargeting:
             window_keypoints=torch.zeros((num_streams, lag + 1, N.NUM_KEYPOINTS, 3), dtype=torch.float32, device=dev),
             window_fixed_qpos=(torch.zeros((num_streams, lag + 1, nf), dtype=torch.float32, device=dev) if nf else None),
             window_qpos=torch.zeros((num_streams, lag + 1, opt.opt_dof), dtype=torch.float32, device=dev),
-            window_len=torch.zeros((num_streams,), dtype=torch.int32, device=dev))
+            window_len=torch.zeros((num_streams,), dtype=torch.int32, device=dev), accel_weight=accel,
+            prev_qpos=torch.zeros((num_streams, opt.opt_dof), dtype=torch.float32, device=dev) if accel else None,
+            has_prev=torch.zeros((num_streams,), dtype=torch.int32, device=dev) if accel else None)
 
     def make_fixed_lag_tape(self, num_streams: int, num_ticks: int, lag: int) -> FixedLagTape:
         """Buffers for recording a `retarget_fixed_lag` call of K ticks on S streams of lag L (`tape=`), the input of
@@ -819,8 +849,8 @@ class SeqRetargeting:
             projected=torch.empty((S, K, len_proj), dtype=torch.uint8, device=dev) if len_proj else None)
 
     def _fixed_lag_call(self, state: FixedLagState, K: int, fill, smooth_weight, stream, tape: Optional[FixedLagTape] = None):
-        """One `dexr_fixed_lag_step` call on `state` with K ticks (`dexr_fixed_lag_step_tape` into `tape` when given);
-        `fill(io, chk)` sets the per-call buffers."""
+        """One `dexr_fixed_lag_step` call on `state` with K ticks (`dexr_fixed_lag_step_tape` into `tape` when given,
+        `dexr_fixed_lag_step_accel` for an accelerated state); `fill(io, chk)` sets the per-call buffers."""
         import torch
 
         opt = self.optimizer
@@ -847,12 +877,23 @@ class SeqRetargeting:
         io.window_len = chk(state.window_len, (S,), torch.int32, "state.window_len")
         io.smooth_weight = -1.0 if smooth_weight is None else float(smooth_weight)
         fill(io, chk)
-        nbytes = int(eng.lib.dexr_fixed_lag_workspace_bytes(eng.handle, S, L))
+        accel = float(state.accel_weight)
+        nbytes = int(eng.lib.dexr_fixed_lag_accel_workspace_bytes(eng.handle, S, L) if accel
+                     else eng.lib.dexr_fixed_lag_workspace_bytes(eng.handle, S, L))
         ws = torch.empty((max(nbytes, 4),), dtype=torch.uint8, device=dev)
         io.workspace, io.workspace_bytes = ws.data_ptr(), nbytes
         s = stream if stream is not None else torch.cuda.current_stream(dev)
         p = opt.params(clip_init=True, lp_alpha=self.low_pass_alpha)
-        if tape is None:
+        if accel:
+            acc = N.DexrFixedLagAccel()
+            acc.accel_weight = accel
+            if state.prev_qpos is None or state.has_prev is None:
+                raise ValueError("an accelerated fixed-lag state needs prev_qpos and has_prev")
+            acc.prev_qpos = chk(state.prev_qpos, (S, n), torch.float32, "state.prev_qpos")
+            acc.has_prev = chk(state.has_prev, (S,), torch.int32, "state.has_prev")
+            N.check(eng.lib.dexr_fixed_lag_step_accel(eng.handle, C.byref(p), C.byref(io), C.byref(acc), S, K,
+                                                      C.c_void_p(s.cuda_stream)), "dexr_fixed_lag_step_accel")
+        elif tape is None:
             N.check(eng.lib.dexr_fixed_lag_step(eng.handle, C.byref(p), C.byref(io), S, K, C.c_void_p(s.cuda_stream)),
                     "dexr_fixed_lag_step")
         else:
@@ -879,6 +920,7 @@ class SeqRetargeting:
         the state are the same bits either way.  Allocates its workspace on the device; nothing is synchronised."""
         import torch
 
+        _refuse_accel_backward(state, "retarget_fixed_lag(tape=...)", tape is not None)
         opt = self.optimizer
         if keypoints.dim() != 4 or tuple(keypoints.shape[2:]) != (N.NUM_KEYPOINTS, 3):
             raise ValueError(f"keypoints must have shape [S,K,21,3], got {tuple(keypoints.shape)}")
@@ -1003,6 +1045,7 @@ class SeqRetargeting:
         by their dexr_fixed_lag_vjp_t names (grad_keypoints, ..., status_out).  Nothing is synchronised."""
         import torch
 
+        _refuse_accel_backward(state0, "retarget_fixed_lag_vjp")
         opt = self.optimizer
         if keypoints.dim() != 4 or tuple(keypoints.shape[2:]) != (N.NUM_KEYPOINTS, 3):
             raise ValueError(f"keypoints must have shape [S,K,21,3], got {tuple(keypoints.shape)}")
@@ -1046,6 +1089,7 @@ class SeqRetargeting:
         grad_window_fixed_qpos or None, grad_window_qpos) of `state0`, the state before the flush."""
         import torch
 
+        _refuse_accel_backward(state0, "flush_fixed_lag_vjp")
         opt = self.optimizer
         S, L = int(state0.last_qpos.shape[0]), int(state0.lag)
         n, dof = opt.opt_dof, opt.robot.dof

@@ -622,6 +622,40 @@ int dexr_fixed_lag_step(const dexr_robot_t* robot, const dexr_params_t* params, 
                         int64_t num_streams, int64_t num_ticks, void* cuda_stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Fixed-lag smoothing with an acceleration penalty: dexr_fixed_lag_step whose window solve is
+ * dexr_smooth_sequences_packed_accel (c = acc->accel_weight) and whose state also carries the frame committed before the
+ * anchor, so that the triple at the window's start is not lost.  State per stream s, in addition to dexr_fixed_lag_t's:
+ *   prev_qpos[s]  p, the frame committed before last_qpos[s], stored raw (unclipped);
+ *   has_prev[s]   0 for a fresh stream, 1 once a frame has been committed (any non-zero value reads as 1).
+ * A tick's solve is exactly smooth_packed_stream<G, ACC = true> on the h+1 window frames anchored at clip(last_qpos), plus,
+ * when has_prev[s] is 1, the triple (clip(p), clip(a), x_0): F gains c |x_0 - 2 clip(a) + clip(p)|^2, which changes only
+ * x_0's gradient, its diagonal block (+2c I) and F_0; p and a are constants.  p is clipped at use, as the anchor is: a
+ * fresh stream's warm start may lie outside clip_lo / clip_hi, and the offline smoother uses clip(a) as frame -1.
+ * On every committed frame (a tick's or a flush's): prev_qpos = last_qpos (the old anchor, raw), has_prev = 1, then
+ * last_qpos = the committed frame.  So a flush of h frames leaves prev_qpos at the second-to-last committed frame.
+ * Consequences: a fresh stream with L >= T-1 plus a flush is dexr_smooth_sequences_packed_accel on the whole clip from the
+ * same anchor, bit for bit (no solve sees a pre-anchor); L = 0 is the causal minimiser of
+ * L_t(x) + w |x - clip(a)|^2 + c |x - 2 clip(a) + clip(p)|^2 (a constant-velocity prior; the first frame of a fresh stream
+ * has no c term); splitting a run into calls, or batching streams, changes no bit.
+ * c is fixed for the life of a state, like the lag; a c = 0 stream uses dexr_fixed_lag_step and has no prev_qpos / has_prev.
+ * A non-finite prev_qpos with has_prev = 1 is a non-finite start of the window solve (DEXR_STATUS_NONFINITE, the warm start
+ * emitted as given; other streams untouched); a commit moves the pre-anchor on.  Missing frames, DexPilot flags, PENDING, MAXITER, window_len clamping, the raw-landmark refusal and asynchrony
+ * are dexr_fixed_lag_step's.  DEXR_E_INVALID for any of dexr_fixed_lag_step's checks, a c that is <= 0 or non-finite,
+ * prev_qpos or has_prev NULL while num_streams > 0, or io->workspace_bytes below
+ * dexr_fixed_lag_accel_workspace_bytes(robot, num_streams, lag): the accel smoother's workspace for S (L+1) frames followed
+ * by S (L+1) int32 status words.  There is no backward through accelerated streams yet.
+ * ------------------------------------------------------------------------------------------- */
+typedef struct dexr_fixed_lag_accel {
+  float accel_weight; /* c: finite, > 0 (c = 0 streams use dexr_fixed_lag_step)                                         */
+  float* prev_qpos;   /* [S,n_var] in/out: the frame committed before last_qpos (raw)                                   */
+  int32_t* has_prev;  /* [S] in/out: 0 fresh, 1 after the first commit                                                  */
+} dexr_fixed_lag_accel_t;
+size_t dexr_fixed_lag_accel_sizeof(void);
+size_t dexr_fixed_lag_accel_workspace_bytes(const dexr_robot_t* robot, int64_t num_streams, int32_t lag);
+int dexr_fixed_lag_step_accel(const dexr_robot_t* robot, const dexr_params_t* params, const dexr_fixed_lag_t* io,
+                              const dexr_fixed_lag_accel_t* acc, int64_t num_streams, int64_t num_ticks, void* cuda_stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Recording a fixed-lag call for its backward: dexr_fixed_lag_step_tape is dexr_fixed_lag_step that also stores, for tick k
  * of stream s, the window minimiser X^k the tick's solve left (tape.qpos[s,k,0..m-1], m the window's length; rows m..L are
  * not written) and the committed DexPilot flags that solve started from (tape.projected[s,k], DexPilot only; NULL
