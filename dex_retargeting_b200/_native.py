@@ -185,6 +185,14 @@ class DexrFixedLagVjp(C.Structure):
     ]
 
 
+class DexrFixedLagAccelVjp(C.Structure):
+    """Mirror of `dexr_fixed_lag_accel_vjp_t`: the acceleration weight, the pre-anchor state before the call and the
+    pre-anchor's cotangents of `dexr_fixed_lag_step_accel_vjp`."""
+
+    _fields_ = [("accel_weight", _f), ("prev_qpos", C.c_void_p), ("has_prev", C.c_void_p), ("grad_prev_qpos_out", C.c_void_p),
+                ("grad_prev_qpos", C.c_void_p)]
+
+
 class DexrGroup(C.Structure):
     """Mirror of `dexr_group_t`: one (robot, batch) group of a mixed-robot launch."""
 
@@ -212,7 +220,8 @@ EXPORTS = [
     "dexr_fixed_lag_tape_sizeof", "dexr_fixed_lag_step_tape", "dexr_fixed_lag_vjp_sizeof",
     "dexr_fixed_lag_vjp_workspace_bytes", "dexr_fixed_lag_step_vjp", "dexr_smooth_accel_workspace_bytes",
     "dexr_smooth_sequences_packed_accel", "dexr_smooth_sequences_packed_accel_vjp", "dexr_fixed_lag_accel_sizeof",
-    "dexr_fixed_lag_accel_workspace_bytes", "dexr_fixed_lag_step_accel",
+    "dexr_fixed_lag_accel_workspace_bytes", "dexr_fixed_lag_step_accel", "dexr_fixed_lag_accel_vjp_sizeof",
+    "dexr_fixed_lag_accel_vjp_workspace_bytes", "dexr_fixed_lag_step_accel_tape", "dexr_fixed_lag_step_accel_vjp",
 ]
 
 _LIB = None
@@ -382,6 +391,20 @@ def load():
                                                   C.POINTER(DexrFixedLagAccel), C.c_int64, C.c_int64, C.c_void_p]
     elif not os.environ.get("DEXR_LIBRARY"):
         raise DexrError(f"{path} does not export dexr_fixed_lag_accel_sizeof: rebuild it "
+                        "(python -m dex_retargeting_b200.build --force)")
+    if hasattr(lib, "dexr_fixed_lag_accel_vjp_sizeof"):
+        lib.dexr_fixed_lag_accel_vjp_sizeof.restype = C.c_size_t
+        if lib.dexr_fixed_lag_accel_vjp_sizeof() != C.sizeof(DexrFixedLagAccelVjp):
+            raise DexrError("dexr_fixed_lag_accel_vjp_t layout mismatch between library and binding (stale DEXR_LIBRARY?)")
+        lib.dexr_fixed_lag_accel_vjp_workspace_bytes.argtypes = [C.c_void_p, C.c_int64, C.c_int32]
+        lib.dexr_fixed_lag_accel_vjp_workspace_bytes.restype = C.c_size_t
+        lib.dexr_fixed_lag_step_accel_tape.argtypes = [C.c_void_p, C.POINTER(DexrParams), C.POINTER(DexrFixedLag),
+                                                       C.POINTER(DexrFixedLagAccel), C.POINTER(DexrFixedLagTape), C.c_int64,
+                                                       C.c_int64, C.c_void_p]
+        lib.dexr_fixed_lag_step_accel_vjp.argtypes = [C.c_void_p, C.POINTER(DexrParams), C.POINTER(DexrFixedLagVjp),
+                                                      C.POINTER(DexrFixedLagAccelVjp), C.c_int64, C.c_int64, C.c_void_p]
+    elif not os.environ.get("DEXR_LIBRARY"):
+        raise DexrError(f"{path} does not export dexr_fixed_lag_accel_vjp_sizeof: rebuild it "
                         "(python -m dex_retargeting_b200.build --force)")
     # (an older A/B library named by DEXR_LIBRARY reads a prefix of the buffer structs -- fields are only ever appended -- so
     # the single-robot entry points still work with it; dexr_solve_frames_multi, whose groups embed the struct, does not)

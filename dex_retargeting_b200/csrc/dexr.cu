@@ -818,6 +818,13 @@ __global__ void __launch_bounds__(kEvalWarps * 32, G == 16 ? 2 : 1) dexr_fixed_l
   fixed_lag_kernel_body<G, false, true>(a, dexr_fixed_lag_tape_t{nullptr, nullptr}, &acc);
 }
 
+// dexr_fixed_lag_step_accel_tape: dexr_fixed_lag_accel_kernel with fixed_lag_tick's recording switched on.
+template <int G>
+__global__ void __launch_bounds__(kEvalWarps * 32, G == 16 ? 2 : 1) dexr_fixed_lag_accel_tape_kernel(
+    const FixedLagArgs a, const dexr_fixed_lag_tape_t tape, const __grid_constant__ dexr_fixed_lag_accel_t acc) {
+  fixed_lag_kernel_body<G, true, true>(a, tape, &acc);
+}
+
 // backpropagation through fixed-lag smoothing: dexr_smooth_vjp_kernel's launch shape, the streams dealt as
 // dexr_fixed_lag_kernel deals them, a stream's ticks walked in reverse on its warp (a 16-lane warp's second group idles)
 struct FixedLagVjpArgs {
@@ -834,8 +841,12 @@ struct FixedLagVjpArgs {
   int pos_off;  // shared memory: each warp's loop state, 2 long longs
 };
 
-template <int G>
-__global__ void __launch_bounds__(kEvalWarps * 32, G == 16 ? 2 : 1) dexr_fixed_lag_vjp_kernel(const FixedLagVjpArgs a) {
+// The body of dexr_fixed_lag_vjp_kernel and dexr_fixed_lag_accel_vjp_kernel; ACC (dexr_fixed_lag_step_accel_vjp): the
+// accelerated window VJP (smooth_vjp_packed_stream<G, true, true>, the window view's c and H_k flags set by the launch) and
+// the fixed_lag_vjp_* helpers' pre-anchor rows and C2, with `acc` and the workspace's `pw`.
+template <int G, bool ACC = false>
+__device__ __forceinline__ void fixed_lag_vjp_kernel_body(const FixedLagVjpArgs& a, const dexr_fixed_lag_accel_vjp_t* acc = nullptr,
+                                                          const FixedLagPreWs* pw = nullptr) {
   load_shared_table(*reinterpret_cast<SharedTable*>(dsmem), a.table);
   __syncthreads();
   constexpr int GPW = 32 / G;
@@ -854,7 +865,7 @@ __global__ void __launch_bounds__(kEvalWarps * 32, G == 16 ? 2 : 1) dexr_fixed_l
   const long long first = (long long)warp * gridDim.x + blockIdx.x;
   if (a.K == 0) {
     for (long long s = first; s < a.S; s += (long long)gridDim.x * kEvalWarps)
-      fixed_lag_vjp_begin(sv, a.io, a.ws, a.dm, s, 0, (threadIdx.x & 31) < G);
+      fixed_lag_vjp_begin<G, ACC>(sv, a.io, a.ws, a.dm, s, 0, (threadIdx.x & 31) < G, acc, pw);
     return;
   }
   if ((threadIdx.x & 31) == 0) {
@@ -863,10 +874,10 @@ __global__ void __launch_bounds__(kEvalWarps * 32, G == 16 ? 2 : 1) dexr_fixed_l
   }
   __syncwarp();
   while (pos()[0] < a.S) {
-    if (pos()[1] == a.K - 1) fixed_lag_vjp_begin(sv, a.io, a.ws, a.dm, pos()[0], a.K, (threadIdx.x & 31) < G);
-    if (fixed_lag_vjp_rebuild(sv, a.io, a.ws, a.dm, a.K, pos(), (threadIdx.x & 31) < G)) {
-      smooth_vjp_packed_stream(sv, a.wio, a.dm, a.wpk, 2 * pos()[0], (threadIdx.x & 31) < G);
-      fixed_lag_vjp_scatter(sv, a.io, a.ws, a.dm, a.K, pos(), (threadIdx.x & 31) < G);
+    if (pos()[1] == a.K - 1) fixed_lag_vjp_begin<G, ACC>(sv, a.io, a.ws, a.dm, pos()[0], a.K, (threadIdx.x & 31) < G, acc, pw);
+    if (fixed_lag_vjp_rebuild<G, ACC>(sv, a.io, a.ws, a.dm, a.K, pos(), (threadIdx.x & 31) < G, acc, pw)) {
+      smooth_vjp_packed_stream<G, ACC, ACC>(sv, a.wio, a.dm, a.wpk, 2 * pos()[0], (threadIdx.x & 31) < G);
+      fixed_lag_vjp_scatter<G, ACC>(sv, a.io, a.ws, a.dm, a.K, pos(), (threadIdx.x & 31) < G, acc, pw);
     }
     if ((threadIdx.x & 31) == 0) {
       volatile long long* const p = pos();
@@ -879,6 +890,19 @@ __global__ void __launch_bounds__(kEvalWarps * 32, G == 16 ? 2 : 1) dexr_fixed_l
     }
     __syncwarp();
   }
+}
+
+template <int G>
+__global__ void __launch_bounds__(kEvalWarps * 32, G == 16 ? 2 : 1) dexr_fixed_lag_vjp_kernel(const FixedLagVjpArgs a) {
+  fixed_lag_vjp_kernel_body<G>(a);
+}
+
+// dexr_fixed_lag_step_accel_vjp: dexr_fixed_lag_vjp_kernel through acceleration-penalised windows (its own kernel, so that
+// the velocity-only one keeps its code; a.ws.smooth holds SmoothAccWs<G> per frame, `pw` the pre-anchor flags and C2).
+template <int G>
+__global__ void __launch_bounds__(kEvalWarps * 32, G == 16 ? 2 : 1) dexr_fixed_lag_accel_vjp_kernel(
+    const FixedLagVjpArgs a, const __grid_constant__ dexr_fixed_lag_accel_vjp_t acc, const __grid_constant__ FixedLagPreWs pw) {
+  fixed_lag_vjp_kernel_body<G, true>(a, &acc, &pw);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -2206,7 +2230,7 @@ extern "C" int dexr_smooth_sequences_packed_accel_vjp(const dexr_robot_t* robot,
 
 // dexr_fixed_lag_step: launch_smooth's CTA and occupancy rule.  `tape`: dexr_fixed_lag_step_tape's recording; `acc`:
 // dexr_fixed_lag_step_accel's pre-anchor state (dexr_fixed_lag_accel_kernel, its own occupancy, the status words after the
-// accel smoother's workspace).
+// accel smoother's workspace); both: dexr_fixed_lag_step_accel_tape (dexr_fixed_lag_accel_tape_kernel).
 template <int G>
 static int launch_fixed_lag(dexr_robot* r, const dexr_params_t* prm, const dexr_fixed_lag_t* io, long long S, int K,
                             cudaStream_t stream, const dexr_fixed_lag_tape_t* tape = nullptr,
@@ -2228,13 +2252,19 @@ static int launch_fixed_lag(dexr_robot* r, const dexr_params_t* prm, const dexr_
   auto kern = dexr_fixed_lag_kernel<G>;
   auto kern_tape = dexr_fixed_lag_tape_kernel<G>;
   auto kern_acc = dexr_fixed_lag_accel_kernel<G>;
+  auto kern_acc_tape = dexr_fixed_lag_accel_tape_kernel<G>;
   CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  if (tape) CUDA_TRY(cudaFuncSetAttribute(kern_tape, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  if (acc) CUDA_TRY(cudaFuncSetAttribute(kern_acc, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  if (tape && !acc) CUDA_TRY(cudaFuncSetAttribute(kern_tape, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  if (acc && !tape) CUDA_TRY(cudaFuncSetAttribute(kern_acc, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  if (acc && tape) CUDA_TRY(cudaFuncSetAttribute(kern_acc_tape, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
   int per_sm = 1;
-  if (int e = acc ? eval_ctas_per_sm(kern_acc, smem, &per_sm) : eval_ctas_per_sm(kern, smem, &per_sm)) return e;
+  if (int e = (acc && tape) ? eval_ctas_per_sm(kern_acc_tape, smem, &per_sm)
+              : acc       ? eval_ctas_per_sm(kern_acc, smem, &per_sm)
+                          : eval_ctas_per_sm(kern, smem, &per_sm))
+    return e;
   const int grid = (int)std::min<long long>(S, (long long)r->num_sms * per_sm);
-  if (acc) kern_acc<<<grid, kEvalWarps * 32, smem, stream>>>(a, *acc);
+  if (acc && tape) kern_acc_tape<<<grid, kEvalWarps * 32, smem, stream>>>(a, *tape, *acc);
+  else if (acc) kern_acc<<<grid, kEvalWarps * 32, smem, stream>>>(a, *acc);
   else if (tape) kern_tape<<<grid, kEvalWarps * 32, smem, stream>>>(a, *tape);
   else kern<<<grid, kEvalWarps * 32, smem, stream>>>(a);
   CUDA_TRY(cudaGetLastError());
@@ -2287,6 +2317,26 @@ extern "C" int dexr_fixed_lag_step_accel(const dexr_robot_t* robot, const dexr_p
                                    : launch_fixed_lag<32>(r, params, io, num_streams, (int)num_ticks, stream, nullptr, acc);
 }
 
+extern "C" int dexr_fixed_lag_step_accel_tape(const dexr_robot_t* robot, const dexr_params_t* params,
+                                              const dexr_fixed_lag_t* io, const dexr_fixed_lag_accel_t* acc,
+                                              const dexr_fixed_lag_tape_t* tape, int64_t num_streams, int64_t num_ticks,
+                                              void* cuda_stream) {
+  if (!robot || !params || !io || !acc || !tape) return fail(DEXR_E_INVALID, "dexr_fixed_lag_step_accel_tape: null argument");
+  if (const char* msg = fixed_lag_io_error(robot->host, *io, *params, num_streams, num_ticks))
+    return fail(DEXR_E_INVALID, "%s", msg);
+  if (const char* msg = fixed_lag_accel_error(robot->host, *io, *acc, num_streams)) return fail(DEXR_E_INVALID, "%s", msg);
+  if (num_ticks > 0)
+    if (const char* msg = fixed_lag_tape_error(robot->host, tape)) return fail(DEXR_E_INVALID, "%s", msg);
+  if (int e = check_params(params)) return e;
+  if (num_streams == 0 || (num_ticks == 0 && !io->flush_count_out)) return 0;
+  DEVICE_SCOPE(robot->device);
+  dexr_robot* r = const_cast<dexr_robot*>(robot);
+  cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
+  const dexr_fixed_lag_tape_t tp{tape->qpos, robot->host.len_proj > 0 ? tape->projected : nullptr};
+  return eval_lanes(r->host) == 16 ? launch_fixed_lag<16>(r, params, io, num_streams, (int)num_ticks, stream, &tp, acc)
+                                   : launch_fixed_lag<32>(r, params, io, num_streams, (int)num_ticks, stream, &tp, acc);
+}
+
 extern "C" size_t dexr_fixed_lag_tape_sizeof(void) { return sizeof(dexr_fixed_lag_tape_t); }
 
 extern "C" int dexr_fixed_lag_step_tape(const dexr_robot_t* robot, const dexr_params_t* params, const dexr_fixed_lag_t* io,
@@ -2307,17 +2357,19 @@ extern "C" int dexr_fixed_lag_step_tape(const dexr_robot_t* robot, const dexr_pa
                                    : launch_fixed_lag<32>(r, params, io, num_streams, (int)num_ticks, stream, &tp);
 }
 
-// dexr_fixed_lag_step_vjp: launch_fixed_lag's CTA and occupancy rule.
+// dexr_fixed_lag_step_vjp: launch_fixed_lag's CTA and occupancy rule.  `acc`: dexr_fixed_lag_step_accel_vjp
+// (dexr_fixed_lag_accel_vjp_kernel, its own occupancy, the accelerated workspace layout and window view).
 template <int G>
 static int launch_fixed_lag_vjp(dexr_robot* r, const dexr_params_t* prm, const dexr_fixed_lag_vjp_t* io, long long S, int K,
-                                cudaStream_t stream) {
+                                cudaStream_t stream, const dexr_fixed_lag_accel_vjp_t* acc = nullptr) {
   FixedLagVjpArgs a{};
   a.table = r->table_dev;
   a.prm = *prm;
   if (!(io->smooth_weight < 0.f)) a.prm.norm_delta = io->smooth_weight;
   a.io = *io;
-  fixed_lag_vjp_layout(r->host, S, io->lag, io->workspace, &a.ws);
-  a.wio = fixed_lag_vjp_window_io(r->host, a.ws);
+  FixedLagPreWs pw{};
+  fixed_lag_vjp_layout(r->host, S, io->lag, io->workspace, &a.ws, acc ? &pw : nullptr);
+  a.wio = acc ? fixed_lag_accel_vjp_window_io(r->host, a.ws, pw, acc->accel_weight) : fixed_lag_vjp_window_io(r->host, a.ws);
   a.wpk = PackedLayout{a.ws.offsets, 2 * S, S * (io->lag + 1)};
   a.S = S;
   a.K = K;
@@ -2327,11 +2379,14 @@ static int launch_fixed_lag_vjp(dexr_robot* r, const dexr_params_t* prm, const d
   a.pos_off = round_up(a.scratch_off + kEvalWarps * GPW * VjpScratch<G>::kFloats * 4, 16);
   const int smem = a.pos_off + kEvalWarps * 2 * (int)sizeof(long long);
   auto kern = dexr_fixed_lag_vjp_kernel<G>;
-  CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  auto kern_acc = dexr_fixed_lag_accel_vjp_kernel<G>;
+  if (acc) CUDA_TRY(cudaFuncSetAttribute(kern_acc, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  else CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
   int per_sm = 1;
-  if (int e = eval_ctas_per_sm(kern, smem, &per_sm)) return e;
+  if (int e = acc ? eval_ctas_per_sm(kern_acc, smem, &per_sm) : eval_ctas_per_sm(kern, smem, &per_sm)) return e;
   const int grid = (int)std::min<long long>(S, (long long)r->num_sms * per_sm);
-  kern<<<grid, kEvalWarps * 32, smem, stream>>>(a);
+  if (acc) kern_acc<<<grid, kEvalWarps * 32, smem, stream>>>(a, *acc, pw);
+  else kern<<<grid, kEvalWarps * 32, smem, stream>>>(a);
   CUDA_TRY(cudaGetLastError());
   {
     std::lock_guard<std::mutex> lk(r->info_mu);
@@ -2358,6 +2413,29 @@ extern "C" int dexr_fixed_lag_step_vjp(const dexr_robot_t* robot, const dexr_par
   cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
   return eval_lanes(r->host) == 16 ? launch_fixed_lag_vjp<16>(r, params, io, num_streams, (int)num_ticks, stream)
                                    : launch_fixed_lag_vjp<32>(r, params, io, num_streams, (int)num_ticks, stream);
+}
+
+extern "C" size_t dexr_fixed_lag_accel_vjp_sizeof(void) { return sizeof(dexr_fixed_lag_accel_vjp_t); }
+
+extern "C" size_t dexr_fixed_lag_accel_vjp_workspace_bytes(const dexr_robot_t* robot, int64_t num_streams, int32_t lag) {
+  return robot ? fixed_lag_accel_vjp_workspace_bytes(robot->host, num_streams, lag) : 0;
+}
+
+extern "C" int dexr_fixed_lag_step_accel_vjp(const dexr_robot_t* robot, const dexr_params_t* params,
+                                             const dexr_fixed_lag_vjp_t* io, const dexr_fixed_lag_accel_vjp_t* acc,
+                                             int64_t num_streams, int64_t num_ticks, void* cuda_stream) {
+  if (!robot || !params || !io || !acc) return fail(DEXR_E_INVALID, "dexr_fixed_lag_step_accel_vjp: null argument");
+  if (const char* msg = fixed_lag_vjp_io_error(robot->host, *io, *params, num_streams, num_ticks))
+    return fail(DEXR_E_INVALID, "%s", msg);
+  if (const char* msg = fixed_lag_accel_vjp_error(robot->host, *io, *acc, num_streams))
+    return fail(DEXR_E_INVALID, "%s", msg);
+  if (int e = check_loss_params(params)) return e;
+  if (num_streams == 0) return 0;
+  DEVICE_SCOPE(robot->device);
+  dexr_robot* r = const_cast<dexr_robot*>(robot);
+  cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
+  return eval_lanes(r->host) == 16 ? launch_fixed_lag_vjp<16>(r, params, io, num_streams, (int)num_ticks, stream, acc)
+                                   : launch_fixed_lag_vjp<32>(r, params, io, num_streams, (int)num_ticks, stream, acc);
 }
 
 extern "C" {

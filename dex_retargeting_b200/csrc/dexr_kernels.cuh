@@ -2819,6 +2819,22 @@ __device__ __forceinline__ float pre_anchor_res(const Solver<G, 0>& sv, const de
   return x - 2.f * a + p;
 }
 
+// The pre-anchor of a fixed-lag window VJP (smooth_vjp_packed_stream<G, true, true>, dexr_fixed_lag_step_accel_vjp, DESIGN.md
+// 3.18).  The window view runs packed stream sc = 2 s only, so row sc + 1 of io.last_qpos holds its pre-anchor (raw) and row
+// sc + 1 of io.grad_last_qpos takes its cotangent; the flags travel in io.workspace_bytes, which the kernel never reads (the
+// device address of an int32 per packed stream), as the forward's pre-anchor state travels in io.cost_out.  Read at each use.
+__device__ __forceinline__ bool pre_anchor_vjp_on(const dexr_smooth_vjp_t& io, long long sc, bool has) {
+  return has && reinterpret_cast<const int32_t*>(io.workspace_bytes)[sc] != 0;
+}
+// pre_anchor_res for the window VJP (`a`: this lane's clip(a)).
+template <int G>
+__device__ __forceinline__ float pre_anchor_vjp_res(const Solver<G, 0>& sv, const dexr_smooth_vjp_t& io, long long sc, int n,
+                                                    float a, float x) {
+  const SharedTable& st = Solver<G, 0>::ST();
+  const float p = fminf(fmaxf(io.last_qpos[(sc + 1) * n + sv.var], st.clip_lo[sv.l]), st.clip_hi[sv.l]);
+  return x - 2.f * a + p;
+}
+
 // The banded block elimination's share of frame t (ACC), between fold_free_block and factor_rows: with the dense coupling
 // E_{t-1} between frames t-1 and t and P = Z_{t-1} E_{t-1} (column per lane, in the kH area),
 //   S_t = D_t - E_{t-1}^T P - c2^2 Z_{t-2},   y_t = y - P^T y_{t-1} - c2 Z_{t-2} y_{t-2},   E_t = b I - c1 P^T
@@ -3183,9 +3199,14 @@ inline const char* smooth_vjp_io_error(const dexr_table_t& t, const dexr_smooth_
 // ACC (dexr_smooth_sequences_packed_accel_vjp): the exact block-pentadiagonal Hessian of F_c (c = io.smooth_weight, as in
 // smooth_packed_stream<G, true>), eliminated as the forward eliminates it with mu = 0; the anchor's cotangent gains
 // 4c v_0 - 2c v_1 when the stream has a second frame.
-template <int G, bool ACC = false>
+// PRE (with ACC; dexr_fixed_lag_step_accel_vjp, DESIGN.md 3.18): a stream with a pre-anchor (pre_anchor_vjp_on) has the
+// forward's triple (clip(p), clip(a), x_0): its share of g_0, +2c on x_0's diagonal block, a non-finite p as a non-finite
+// stream, 4c v_0 more in the anchor's cotangent (after the terms above) and -2c v_0 as p's cotangent where the clip passes
+// p (0 without a pre-anchor).
+template <int G, bool ACC = false, bool PRE = false>
 __device__ __forceinline__ void smooth_vjp_packed_stream(Solver<G, 0>& sv, const dexr_smooth_vjp_t& io, const Dims& dm,
                                                          const PackedLayout& pk, long long si, bool owner) {
+  static_assert(ACC || !PRE, "the pre-anchor is a triple of the acceleration penalty");
   using W = typename SmoothWsOf<G, ACC>::type;
   constexpr int NP = G;
   const SharedTable& st = Solver<G, 0>::ST();
@@ -3233,6 +3254,8 @@ __device__ __forceinline__ void smooth_vjp_packed_stream(Solver<G, 0>& sv, const
   auto raw_anchor = [&]() { return (has && isvar && anchor) ? io.last_qpos[sc * n + sv.var] : 0.f; };
   auto clipped_anchor = [&]() { return fminf(fmaxf(raw_anchor(), st.clip_lo[l]), st.clip_hi[l]); };
   bool nonfinite = !isfinite(raw_anchor());
+  if constexpr (PRE)
+    if (isvar && pre_anchor_vjp_on(io, sc, has)) nonfinite = nonfinite || !isfinite(io.last_qpos[(sc + 1) * n + sv.var]);
 
   // ---- forward sweep: the elimination of H V = G.  G_t waits in the workspace's kG slot while the frame is evaluated, and
   // only the smoothness gradient of the neighbours stays in registers (the 16-lane kernel has 128 of them)
@@ -3277,6 +3300,9 @@ __device__ __forceinline__ void smooth_vjp_packed_stream(Solver<G, 0>& sv, const
         if (at.left) xn2 = io.qpos[(fr + 2) * n + sv.var];
       }
       if (isvar) g += at.grad(io.smooth_weight, xp2, xp, x, xn_, xn2);
+      if constexpr (PRE)
+        if (t == 0 && isvar && pre_anchor_vjp_on(io, sc, has))  // the triple (p, a, x_0); xp is clip(a) at t = 0
+          g += 2.f * io.smooth_weight * pre_anchor_vjp_res(sv, io, sc, n, xp, x);
     }
     const bool at_bound = isvar && ((x <= sv.lo && g > -kGradNoise) || (x >= sv.hi && g < kGradNoise));
     const bool free_ = live && isvar && !at_bound;
@@ -3287,6 +3313,9 @@ __device__ __forceinline__ void smooth_vjp_packed_stream(Solver<G, 0>& sv, const
                                                     w2 * (float)((has_prev ? 1 : 0) + (has_next ? 1 : 0))));
     else
       fold_free_block(sv, dm, A, free_, fmask, w2 * (float)((has_prev ? 1 : 0) + (has_next ? 1 : 0)));
+    if constexpr (PRE)
+      if (t == 0 && free_ && pre_anchor_vjp_on(io, sc, has))  // the triple (p, a, x_0): +2c on x_0's diagonal
+        A[l * (NP + 1) + l] += 2.f * io.smooth_weight;
     float y = (free_ && live) ? wt[W::kG + l] : 0.f;
     if constexpr (ACC)
       y = accel_eliminate<G, W>(sv, dof, A, wt, t, live, free_, fmask, y, yprev,
@@ -3390,6 +3419,16 @@ __device__ __forceinline__ void smooth_vjp_packed_stream(Solver<G, 0>& sv, const
         const float v1 = static_cast<const float*>(io.workspace)[(long long)(f0 + 1) * W::kFloats + W::kX + l];
         ga = fmaf(2.f * io.smooth_weight, fmaf(2.f, v0, -v1), ga);
       }
+    }
+    if constexpr (PRE) {  // the triple (p, a, x_0): 4c v_0 more for a; -2c v_0 for p where the clip passes p
+      float gp = 0.f;
+      if (pre_anchor_vjp_on(io, sc, has)) {
+        const float pr = io.last_qpos[(sc + 1) * n + sv.var];
+        const bool ppass = pr >= st.clip_lo[l] && pr <= st.clip_hi[l];
+        if (!nonfinite && !bad && passes) ga = fmaf(4.f * io.smooth_weight, v0, ga);
+        gp = nonfinite ? __int_as_float(0x7fc00000) : ((bad || !ppass) ? 0.f : -2.f * io.smooth_weight * v0);
+      }
+      io.grad_last_qpos[(sc + 1) * n + sv.var] = gp;
     }
     io.grad_last_qpos[sc * n + sv.var] = has ? ga : 0.f;
   }
@@ -3654,11 +3693,22 @@ struct FixedLagVjpWs {
   uint8_t* flags;    // [2S,len_proj] row 2s: the flags W_k's solve started from
 };
 
-// Lays the workspace of S streams of lag L out from `base` (may be nullptr) into `w`; returns its size in bytes.
-inline size_t fixed_lag_vjp_layout(const dexr_table_t& t, long long S, long long lag, void* base, FixedLagVjpWs* w) {
+// The accelerated backward's workspace after FixedLagVjpWs's arrays (dexr_fixed_lag_step_accel_vjp): there `smooth` holds
+// SmoothAccWs<G>::kFloats per frame, row 2s + 1 of `anchor` the pre-anchor P_k of stream s's window and row 2s + 1 of
+// `ganchor` its cotangent, and `abar` is C1.
+struct FixedLagPreWs {
+  int32_t* has;  // [2S] entry 2s: H_k (the window VJP's io.workspace_bytes, pre_anchor_vjp_on)
+  float* cbar2;  // [S,n_var] C2, the carried cotangent of X^{k-1}[0]
+};
+
+// Lays the workspace of S streams of lag L out from `base` (may be nullptr) into `w`; returns its size in bytes.  `pw`
+// (non-null: dexr_fixed_lag_step_accel_vjp's layout): the accel smoother's frames and the FixedLagPreWs arrays after the rest.
+inline size_t fixed_lag_vjp_layout(const dexr_table_t& t, long long S, long long lag, void* base, FixedLagVjpWs* w,
+                                   FixedLagPreWs* pw = nullptr) {
   if (S <= 0 || lag < 0 || lag > DEXR_FIXED_LAG_MAX) return 0;
   const long long F = S * (lag + 1);
-  const int floats = eval_lanes(t) == 16 ? SmoothWs<16>::kFloats : SmoothWs<32>::kFloats;
+  const int floats = pw ? (eval_lanes(t) == 16 ? SmoothAccWs<16>::kFloats : SmoothAccWs<32>::kFloats)
+                        : (eval_lanes(t) == 16 ? SmoothWs<16>::kFloats : SmoothWs<32>::kFloats);
   char* const b = static_cast<char*>(base);
   size_t off = 0;
   auto take = [&](size_t bytes) {
@@ -3681,6 +3731,10 @@ inline size_t fixed_lag_vjp_layout(const dexr_table_t& t, long long S, long long
   r.ganchor = static_cast<float*>(take((size_t)(2 * S) * t.n_var * sizeof(float)));
   r.abar = static_cast<float*>(take((size_t)S * t.n_var * sizeof(float)));
   r.flags = static_cast<uint8_t*>(take((size_t)(2 * S) * t.len_proj));
+  if (pw) {
+    pw->has = static_cast<int32_t*>(take((size_t)(2 * S) * sizeof(int32_t)));
+    pw->cbar2 = static_cast<float*>(take((size_t)S * t.n_var * sizeof(float)));
+  }
   if (w) *w = r;
   return off;
 }
@@ -3688,6 +3742,12 @@ inline size_t fixed_lag_vjp_layout(const dexr_table_t& t, long long S, long long
 // dexr_fixed_lag_vjp_workspace_bytes.
 inline size_t fixed_lag_vjp_workspace_bytes(const dexr_table_t& t, long long S, long long lag) {
   return fixed_lag_vjp_layout(t, S, lag, nullptr, nullptr);
+}
+
+// dexr_fixed_lag_accel_vjp_workspace_bytes.
+inline size_t fixed_lag_accel_vjp_workspace_bytes(const dexr_table_t& t, long long S, long long lag) {
+  FixedLagPreWs pw;
+  return fixed_lag_vjp_layout(t, S, lag, nullptr, nullptr, &pw);
 }
 
 // The smoother VJP's view of a laid-out workspace: packed clips of the rebuilt windows.
@@ -3706,6 +3766,16 @@ inline dexr_smooth_vjp_t fixed_lag_vjp_window_io(const dexr_table_t& t, const Fi
   v.grad_fixed_qpos = t.n_fixed > 0 ? w.gfixed : nullptr;
   v.grad_last_qpos = w.ganchor;
   v.status_out = w.status;
+  return v;
+}
+
+// The accelerated window VJP's view (smooth_vjp_packed_stream<G, true, true>): c in smooth_weight, the H_k flags in
+// workspace_bytes (pre_anchor_vjp_on).
+inline dexr_smooth_vjp_t fixed_lag_accel_vjp_window_io(const dexr_table_t& t, const FixedLagVjpWs& w, const FixedLagPreWs& pw,
+                                                       float accel_weight) {
+  dexr_smooth_vjp_t v = fixed_lag_vjp_window_io(t, w);
+  v.smooth_weight = accel_weight;
+  v.workspace_bytes = reinterpret_cast<size_t>(pw.has);
   return v;
 }
 
@@ -3737,6 +3807,17 @@ inline const char* fixed_lag_vjp_io_error(const dexr_table_t& t, const dexr_fixe
   return nullptr;
 }
 
+// The extra argument checks of dexr_fixed_lag_step_accel_vjp (after fixed_lag_vjp_io_error): nullptr, or what is wrong.
+inline const char* fixed_lag_accel_vjp_error(const dexr_table_t& t, const dexr_fixed_lag_vjp_t& io,
+                                             const dexr_fixed_lag_accel_vjp_t& acc, long long S) {
+  if (!(acc.accel_weight > 0.f && acc.accel_weight <= 3.0e38f))
+    return "accel_weight must be finite and > 0 (c = 0 streams use dexr_fixed_lag_step_vjp)";
+  if (S > 0 && (!acc.prev_qpos || !acc.has_prev)) return "prev_qpos and has_prev (the state before the call) are required";
+  if (S > 0 && io.workspace_bytes < fixed_lag_accel_vjp_workspace_bytes(t, S, io.lag))
+    return "workspace smaller than dexr_fixed_lag_accel_vjp_workspace_bytes(robot, num_streams, lag)";
+  return nullptr;
+}
+
 // Where a stream's call ends (group-uniform): h0 the held frames at the start, hend those held after the ticks (before a
 // flush), cend the frames committed by then (final slot i holds input frame cend + i), elast whether the last tick emitted
 // and `route` where grad_last_qpos_out goes: 0 the incoming anchor, 1 slot 0 of the last window, 2 its last held slot.
@@ -3752,6 +3833,15 @@ __device__ __forceinline__ FixedLagEnd fixed_lag_end(int h0_raw, int L, int K, b
   e.cend = e.h0 + K - L > 0 ? e.h0 + K - L : 0;
   e.route = (flushed && e.hend > 0) ? 2 : (e.elast ? 1 : 0);
   return e;
+}
+
+// Where grad_prev_qpos_out goes (dexr_fixed_lag_step_accel_vjp): the final prev_qpos is commit i = N - 2 of the call's N =
+// cend + (flushed ? hend : 0) commits, the incoming pre-anchor and anchor counting as commits -2 and -1.  0: the incoming
+// pre-anchor (grad_prev_qpos), 1: the incoming anchor (grad_last_qpos), 2: X^{K-2}[0] (C2 at the start), 3: X^{K-1}[0]
+// (slot 0 of the last window), 4: the flushed slot hend - 2.
+__device__ __forceinline__ int fixed_lag_pre_route(const FixedLagEnd& e, bool flushed) {
+  const int i = e.cend + (flushed ? e.hend : 0) - 2;
+  return i == -2 ? 0 : (i == -1 ? 1 : (i >= e.cend ? 4 : (i == e.cend - 1 ? 3 : 2)));
 }
 
 // smooth_vjp_packed_stream's cotangent of a var lane: M^T r (r: this lane's joint's robot_qpos cotangent, the mimic
@@ -3782,11 +3872,15 @@ __device__ __forceinline__ float fixed_lag_fold(const Solver<G, 0>& sv, const Di
 // final state's keypoint and fixed-joint cotangents onto the input frames their held slots hold (the flushed rows' fixed-joint
 // share too: those frames' sums start with it, so a chunked run gives the same bits; unlike the window VJP's direct term
 // it is kept on a NOT_PD window or a missing frame, see dexr.h), the anchor's own cotangent when it routes there, the carried abar zeroed.
-// With K = 0 the flush rows are the incoming held slots of window_qpos.  `owner` as in fixed_lag_tick.
-template <int G>
+// With K = 0 the flush rows are the incoming held slots of window_qpos.  `owner` as in fixed_lag_tick.  ACC
+// (dexr_fixed_lag_step_accel_vjp, with `acc` and the workspace's `pw`): grad_prev_qpos_out goes where fixed_lag_pre_route
+// sends it (grad_last_qpos or grad_prev_qpos written with it, C2 started with it, or a flushed slot's sum), C2 zeroed
+// otherwise; the last window's slot 0 takes it in fixed_lag_vjp_rebuild.
+template <int G, bool ACC = false>
 __device__ __forceinline__ void fixed_lag_vjp_begin(const Solver<G, 0>& sv, const dexr_fixed_lag_vjp_t& io,
                                                     const FixedLagVjpWs& ws, const Dims& dm, long long s, int K,
-                                                    bool owner) {
+                                                    bool owner, const dexr_fixed_lag_accel_vjp_t* acc = nullptr,
+                                                    const FixedLagPreWs* pw = nullptr) {
   constexpr int KP = 3 * DEXR_NUM_KEYPOINTS;
   const int l = sv.l, n = dm.n_var, nf = dm.n_fixed, dof = dm.dof, L = io.lag, W1 = L + 1;
   const bool isvar = sv.var >= 0;
@@ -3808,6 +3902,13 @@ __device__ __forceinline__ void fixed_lag_vjp_begin(const Solver<G, 0>& sv, cons
       if (io.grad_last_qpos)
         io.grad_last_qpos[s * n + sv.var] = (e.route == 0 && io.grad_last_qpos_out) ? io.grad_last_qpos_out[s * n + sv.var] : 0.f;
       ws.abar[s * n + sv.var] = 0.f;
+      if constexpr (ACC) {  // (route 1 is never the anchor's route 0: at most one of the two writes grad_last_qpos)
+        const int pr = fixed_lag_pre_route(e, io.flushed != 0);
+        const float gp = acc->grad_prev_qpos_out ? acc->grad_prev_qpos_out[s * n + sv.var] : 0.f;
+        if (pr == 1 && io.grad_last_qpos) io.grad_last_qpos[s * n + sv.var] = gp;
+        if (acc->grad_prev_qpos) acc->grad_prev_qpos[s * n + sv.var] = pr == 0 ? gp : 0.f;
+        pw->cbar2[s * n + sv.var] = pr == 2 ? gp : 0.f;
+      }
     }
     // the final state's held slots: slot i holds input frame g = cend + i (held at the start when g < h0)
     for (int i = 0; i < e.hend; ++i) {
@@ -3838,6 +3939,9 @@ __device__ __forceinline__ void fixed_lag_vjp_begin(const Solver<G, 0>& sv, cons
         q = io.grad_window_qpos_out ? io.grad_window_qpos_out[(s * W1 + j) * n + sv.var] : 0.f;
         q += (io.flushed && io.grad_flush_qpos) ? io.grad_flush_qpos[(s * L + j) * n + sv.var] : 0.f;
         if (e.route == 2 && j == e.h0 - 1 && io.grad_last_qpos_out) q += io.grad_last_qpos_out[s * n + sv.var];
+        if constexpr (ACC)
+          if (fixed_lag_pre_route(e, io.flushed != 0) == 4 && j == e.h0 - 2 && acc->grad_prev_qpos_out)
+            q += acc->grad_prev_qpos_out[s * n + sv.var];
       }
       const float gb = fixed_lag_fold(sv, dm, r, q);
       if (owner && isvar && io.grad_window_qpos) io.grad_window_qpos[(s * W1 + j) * n + sv.var] = gb;
@@ -3848,11 +3952,15 @@ __device__ __forceinline__ void fixed_lag_vjp_begin(const Solver<G, 0>& sv, cons
 
 // Rebuilds the window of tick pos[1] of stream pos[0] of dexr_fixed_lag_step_vjp in the workspace (frames, fixed joints,
 // point, anchor, flags and the slot cotangents, see dexr.h) when the tick is differentiated -- it emits or is the last --
-// and returns whether it is (group-uniform).  `owner` as in fixed_lag_tick.
-template <int G>
+// and returns whether it is (group-uniform).  `owner` as in fixed_lag_tick.  ACC: also the pre-anchor P_k (row 2s + 1 of
+// ws.anchor: prev_qpos when c_k = 0, last_qpos when c_k = 1, X^{k-2}[0] otherwise) and H_k (has_prev when c_k = 0, else 1),
+// and grad_prev_qpos_out on the slot fixed_lag_pre_route gives it.
+template <int G, bool ACC = false>
 __device__ __forceinline__ bool fixed_lag_vjp_rebuild(const Solver<G, 0>& sv, const dexr_fixed_lag_vjp_t& io,
                                                       const FixedLagVjpWs& ws, const Dims& dm, int K,
-                                                      const volatile long long* pos, bool owner) {
+                                                      const volatile long long* pos, bool owner,
+                                                      const dexr_fixed_lag_accel_vjp_t* acc = nullptr,
+                                                      const FixedLagPreWs* pw = nullptr) {
   constexpr int KP = 3 * DEXR_NUM_KEYPOINTS;
   const int l = sv.l, n = dm.n_var, nf = dm.n_fixed, dof = dm.dof, L = io.lag, W1 = L + 1;
   const long long s = pos[0];
@@ -3886,10 +3994,16 @@ __device__ __forceinline__ bool fixed_lag_vjp_rebuild(const Solver<G, 0>& sv, co
           q = io.grad_qpos ? io.grad_qpos[t * n + sv.var] : 0.f;
           if (!last) q += ws.abar[s * n + sv.var];
           else if (e.route == 1 && io.grad_last_qpos_out) q += io.grad_last_qpos_out[s * n + sv.var];
+          if constexpr (ACC)  // (route 3: the anchor's route is 2, so nothing else was added)
+            if (last && fixed_lag_pre_route(e, io.flushed != 0) == 3 && acc->grad_prev_qpos_out)
+              q += acc->grad_prev_qpos_out[s * n + sv.var];
         } else if (tail) {
           q = io.grad_window_qpos_out ? io.grad_window_qpos_out[(w0 + i) * n + sv.var] : 0.f;
           q += (io.flushed && io.grad_flush_qpos) ? io.grad_flush_qpos[(s * L + i) * n + sv.var] : 0.f;
           if (e.route == 2 && i == e.hend - 1 && io.grad_last_qpos_out) q += io.grad_last_qpos_out[s * n + sv.var];
+          if constexpr (ACC)
+            if (fixed_lag_pre_route(e, io.flushed != 0) == 4 && i == e.hend - 2 && acc->grad_prev_qpos_out)
+              q += acc->grad_prev_qpos_out[s * n + sv.var];
         }
         ws.gq[(w0 + j) * n + sv.var] = q;
       }
@@ -3901,6 +4015,12 @@ __device__ __forceinline__ bool fixed_lag_vjp_rebuild(const Solver<G, 0>& sv, co
       }
     }
     if (isvar) ws.anchor[2 * s * n + sv.var] = c0 == 0 ? io.last_qpos[s * n + sv.var] : io.tape.qpos[((t - 1) * W1) * n + sv.var];
+    if constexpr (ACC) {
+      if (isvar)
+        ws.anchor[(2 * s + 1) * n + sv.var] = c0 == 0 ? acc->prev_qpos[s * n + sv.var]
+                                              : (c0 == 1 ? io.last_qpos[s * n + sv.var] : io.tape.qpos[((t - 2) * W1) * n + sv.var]);
+      if (l == 0) pw->has[2 * s] = c0 == 0 ? (acc->has_prev[s] != 0 ? 1 : 0) : 1;
+    }
     if (l < dm.len_proj) ws.flags[2 * s * dm.len_proj + l] = io.tape.projected[t * dm.len_proj + l];
     if (l == 0) {
       ws.offsets[2 * s] = w0;
@@ -3913,11 +4033,14 @@ __device__ __forceinline__ bool fixed_lag_vjp_rebuild(const Solver<G, 0>& sv, co
 
 // After the window VJP of tick pos[1] of stream pos[0]: its frames' cotangents added to the input frames they came from, its
 // anchor cotangent carried to the previous tick's slot 0 (c_k >= 1) or added to grad_last_qpos (c_k = 0), the emitted
-// frame's status.
-template <int G>
+// frame's status.  ACC, with ga the window's anchor cotangent and gp its pre-anchor's: c_k >= 1: C1 = C2 + ga; c_k = 0:
+// grad_last_qpos += ga; then c_k >= 2: C2 = gp; c_k = 1: grad_last_qpos += gp; c_k = 0: grad_prev_qpos += gp.
+template <int G, bool ACC = false>
 __device__ __forceinline__ void fixed_lag_vjp_scatter(const Solver<G, 0>& sv, const dexr_fixed_lag_vjp_t& io,
                                                       const FixedLagVjpWs& ws, const Dims& dm, int K,
-                                                      const volatile long long* pos, bool owner) {
+                                                      const volatile long long* pos, bool owner,
+                                                      const dexr_fixed_lag_accel_vjp_t* acc = nullptr,
+                                                      const FixedLagPreWs* pw = nullptr) {
   constexpr int KP = 3 * DEXR_NUM_KEYPOINTS;
   const int l = sv.l, n = dm.n_var, nf = dm.n_fixed, L = io.lag, W1 = L + 1;
   const long long s = pos[0];
@@ -3938,7 +4061,20 @@ __device__ __forceinline__ void fixed_lag_vjp_scatter(const Solver<G, 0>& sv, co
       float* const df = held ? io.grad_window_fixed_qpos : io.grad_fixed_qpos;
       if (fixedi >= 0 && df) df[row * nf + fixedi] += ws.gfixed[(w0 + j) * nf + fixedi];
     }
-    if (sv.var >= 0) {
+    if constexpr (ACC) {
+      if (sv.var >= 0) {
+        const float ab = ws.ganchor[2 * s * n + sv.var], gp = ws.ganchor[(2 * s + 1) * n + sv.var];
+        float* const c2 = pw->cbar2 + s * n + sv.var;
+        if (c0 > 0) ws.abar[s * n + sv.var] = *c2 + ab;
+        else if (io.grad_last_qpos) io.grad_last_qpos[s * n + sv.var] += ab;
+        if (c0 > 1) *c2 = gp;
+        else if (c0 == 1) {
+          if (io.grad_last_qpos) io.grad_last_qpos[s * n + sv.var] += gp;
+        } else if (acc->grad_prev_qpos) {
+          acc->grad_prev_qpos[s * n + sv.var] += gp;
+        }
+      }
+    } else if (sv.var >= 0) {
       const float ab = ws.ganchor[2 * s * n + sv.var];
       if (c0 > 0) ws.abar[s * n + sv.var] = ab;
       else if (io.grad_last_qpos) io.grad_last_qpos[s * n + sv.var] += ab;

@@ -268,8 +268,9 @@ def _fixed_lag_copy(state):
     """A detached copy of a FixedLagState (the forward updates its state in place; autograd keeps the original)."""
     from .seq_retarget import FixedLagState
 
-    return FixedLagState(lag=state.lag, **{k: (None if getattr(state, k) is None else getattr(state, k).detach().clone())
-                                           for k in FixedLagState._FIELDS})
+    return FixedLagState(lag=state.lag, accel_weight=float(state.accel_weight),
+                         **{k: (None if getattr(state, k) is None else getattr(state, k).detach().clone())
+                            for k in FixedLagState._FIELDS})
 
 
 class _DifferentiableRetargetFixedLag(torch.autograd.Function):
@@ -309,7 +310,7 @@ def differentiable_retarget_fixed_lag(seq, keypoints, state, fixed_qpos=None, *,
     stream backpropagate across call boundaries (detach the state for truncated backpropagation).  backward() is one
     `retarget_fixed_lag_vjp` launch: each emitting window's smoother VJP, the anchor chain through the committed frames.
     PENDING rows (NaN) get no gradient.  The DexPilot flags and `smooth_weight` are not differentiated.  A state with an
-    acceleration penalty is refused (ValueError): there is no backward through it yet."""
+    acceleration penalty is refused (ValueError): its backward is `differentiable_retarget_fixed_lag_accel`."""
     from .seq_retarget import FixedLagState, _refuse_accel_backward
 
     _refuse_accel_backward(state, "differentiable_retarget_fixed_lag")
@@ -351,7 +352,7 @@ def differentiable_flush_fixed_lag(seq, state):
     """(robot_qpos [S,L,dof], qpos [S,L,opt_dof], count [S], new_state) = `seq.flush_fixed_lag(state)`, differentiable in
     the state's `last_qpos` and window tensors (the flushed rows are its held slots of window_qpos).  `state` is not
     modified; the returned state carries the graph as `differentiable_retarget_fixed_lag`'s does.  A state with an
-    acceleration penalty is refused (ValueError), as there."""
+    acceleration penalty is refused (ValueError), as there: its backward is `differentiable_flush_fixed_lag_accel`."""
     from .seq_retarget import FixedLagState, _refuse_accel_backward
 
     _refuse_accel_backward(state, "differentiable_flush_fixed_lag")
@@ -361,3 +362,114 @@ def differentiable_flush_fixed_lag(seq, state):
     new = cfg["new_state"]
     return rq, q, count, FixedLagState(lag=new.lag, last_qpos=last, projected=new.projected, window_keypoints=wkp,
                                        window_fixed_qpos=wfix, window_qpos=wq, window_len=new.window_len)
+
+
+def _accel_weight_of(state, what):
+    """The state's acceleration weight as a float: it is not differentiated, so a tensor that requires grad is refused."""
+    c = state.accel_weight
+    if isinstance(c, torch.Tensor):
+        if c.requires_grad:
+            raise ValueError(f"{what}: accel_weight requires grad, but fixed-lag smoothing is not differentiated in it: "
+                             "detach it")
+        c = float(c)
+    if not c:
+        raise ValueError(f"{what}: the state has no acceleration penalty (accel_weight = 0): use "
+                         f"{what.replace('_accel', '')}")
+    return float(c)
+
+
+def _accel_copy(state, c):
+    new = _fixed_lag_copy(state)
+    new.accel_weight = c
+    return new
+
+
+class _DifferentiableRetargetFixedLagAccel(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, keypoints, fixed_qpos, last_qpos, window_keypoints, window_fixed_qpos, window_qpos, prev_qpos, seq, cfg):
+        state0 = _accel_copy(cfg["state"], cfg["accel_weight"])
+        new = _fixed_lag_copy(state0)
+        S, K = int(keypoints.shape[0]), int(keypoints.shape[1])
+        tape = seq.make_fixed_lag_tape(S, K, state0.lag, accel_weight=state0.accel_weight)
+        kp = keypoints.detach().contiguous()
+        fixed = None if fixed_qpos is None else fixed_qpos.detach().contiguous()
+        rq, q, status = seq.retarget_fixed_lag(kp, new, fixed_qpos=fixed, smooth_weight=cfg["smooth_weight"], tape=tape)
+        ctx.seq, ctx.tape, ctx.state0, ctx.smooth_weight = seq, tape, state0, cfg["smooth_weight"]
+        ctx.save_for_backward(kp, fixed)
+        ctx.set_materialize_grads(False)
+        ctx.mark_non_differentiable(status)
+        cfg["new_state"] = new
+        return (rq, q, status, new.last_qpos, new.window_keypoints, new.window_fixed_qpos, new.window_qpos,
+                new.prev_qpos)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g_rq, g_q, _g_status, g_last, g_wkp, g_wfix, g_wq, g_prev):
+        kp, fixed = ctx.saved_tensors
+        c = (lambda g: None if g is None else g.contiguous())
+        g_kp, g_fixed, g_last0, g_wkp0, g_wfix0, g_wq0, _, g_prev0 = ctx.seq.retarget_fixed_lag_accel_vjp(
+            kp, ctx.tape, ctx.state0, fixed_qpos=fixed, grad_qpos=c(g_q), grad_robot_qpos=c(g_rq),
+            grad_last_qpos_out=c(g_last), grad_prev_qpos_out=c(g_prev), grad_window_qpos_out=c(g_wq),
+            grad_window_keypoints_out=c(g_wkp), grad_window_fixed_qpos_out=c(g_wfix), smooth_weight=ctx.smooth_weight)
+        return g_kp, g_fixed, g_last0, g_wkp0, g_wfix0, g_wq0, g_prev0, None, None
+
+
+def _accel_state_out(new, last, wkp, wfix, wq, prev):
+    from .seq_retarget import FixedLagState
+
+    return FixedLagState(lag=new.lag, last_qpos=last, projected=new.projected, window_keypoints=wkp, window_fixed_qpos=wfix,
+                         window_qpos=wq, window_len=new.window_len, accel_weight=new.accel_weight, prev_qpos=prev,
+                         has_prev=new.has_prev)
+
+
+def differentiable_retarget_fixed_lag_accel(seq, keypoints, state, fixed_qpos=None, *, smooth_weight=None):
+    """`differentiable_retarget_fixed_lag` for an accelerated state (`make_fixed_lag_state(S, L, accel_weight=c)`, c > 0):
+    (robot_qpos, qpos, status, new_state) = `seq.retarget_fixed_lag(keypoints, state, ...)`, differentiable in
+    `keypoints`, `fixed_qpos` and the state's `last_qpos`, `prev_qpos` and window tensors.  The returned state carries
+    accel_weight, has_prev and the graph through last_qpos, prev_qpos and the windows, so chunks backpropagate across call
+    boundaries.  backward() is one `retarget_fixed_lag_accel_vjp` launch.  The DexPilot flags, `smooth_weight`, c and
+    has_prev are not differentiated (a c or smooth_weight tensor that requires grad is refused)."""
+    if isinstance(smooth_weight, torch.Tensor):
+        if smooth_weight.requires_grad:
+            raise ValueError("smooth_weight requires grad, but fixed-lag smoothing is not differentiated in it: detach it")
+        smooth_weight = float(smooth_weight)
+    accel = _accel_weight_of(state, "differentiable_retarget_fixed_lag_accel")
+    cfg = dict(state=state, smooth_weight=smooth_weight, accel_weight=accel)
+    rq, q, status, last, wkp, wfix, wq, prev = _DifferentiableRetargetFixedLagAccel.apply(
+        keypoints, fixed_qpos, state.last_qpos, state.window_keypoints, state.window_fixed_qpos, state.window_qpos,
+        state.prev_qpos, seq, cfg)
+    return rq, q, status, _accel_state_out(cfg["new_state"], last, wkp, wfix, wq, prev)
+
+
+class _DifferentiableFlushFixedLagAccel(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, last_qpos, window_keypoints, window_fixed_qpos, window_qpos, prev_qpos, seq, cfg):
+        state0 = _accel_copy(cfg["state"], cfg["accel_weight"])
+        new = _fixed_lag_copy(state0)
+        rq, q, count = seq.flush_fixed_lag(new)
+        ctx.seq, ctx.state0 = seq, state0
+        ctx.set_materialize_grads(False)
+        ctx.mark_non_differentiable(count)
+        cfg["new_state"] = new
+        return rq, q, count, new.last_qpos, new.window_keypoints, new.window_fixed_qpos, new.window_qpos, new.prev_qpos
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g_rq, g_q, _g_count, g_last, g_wkp, g_wfix, g_wq, g_prev):
+        c = (lambda g: None if g is None else g.contiguous())
+        g_last0, g_wkp0, g_wfix0, g_wq0, g_prev0 = ctx.seq.flush_fixed_lag_accel_vjp(
+            ctx.state0, grad_qpos=c(g_q), grad_robot_qpos=c(g_rq), grad_last_qpos_out=c(g_last),
+            grad_prev_qpos_out=c(g_prev), grad_window_qpos_out=c(g_wq), grad_window_keypoints_out=c(g_wkp),
+            grad_window_fixed_qpos_out=c(g_wfix))
+        return g_last0, g_wkp0, g_wfix0, g_wq0, g_prev0, None, None
+
+
+def differentiable_flush_fixed_lag_accel(seq, state):
+    """`differentiable_flush_fixed_lag` for an accelerated state: differentiable in the state's `last_qpos`, `prev_qpos`
+    and window tensors; the returned state carries accel_weight, has_prev and the graph as
+    `differentiable_retarget_fixed_lag_accel`'s does."""
+    accel = _accel_weight_of(state, "differentiable_flush_fixed_lag_accel")
+    cfg = dict(state=state, accel_weight=accel)
+    rq, q, count, last, wkp, wfix, wq, prev = _DifferentiableFlushFixedLagAccel.apply(
+        state.last_qpos, state.window_keypoints, state.window_fixed_qpos, state.window_qpos, state.prev_qpos, seq, cfg)
+    return rq, q, count, _accel_state_out(cfg["new_state"], last, wkp, wfix, wq, prev)

@@ -16,7 +16,8 @@ end (`PackedStreams`, the cu_seqlens layout): recorded clips of any length in on
 `smooth_packed_sequences()` solves every frame of each packed clip jointly (`dexr_smooth_sequences_packed`): the offline
 trajectory, with no lag and with dropped frames filled in.  `retarget_fixed_lag()` brings it to live streams
 (`dexr_fixed_lag_step`, `FixedLagState`): each new frame re-solves the last L+1 frames jointly and emits the frame L ticks
-back; a state made with `accel_weight` also penalises acceleration there (`dexr_fixed_lag_step_accel`).
+back; a state made with `accel_weight` also penalises acceleration there (`dexr_fixed_lag_step_accel`), and
+`retarget_fixed_lag_accel_vjp` backpropagates through it.
 """
 from __future__ import annotations
 
@@ -136,11 +137,24 @@ class FixedLagState:
 
 
 def _refuse_accel_backward(state: FixedLagState, what: str, taped: bool = True):
-    """The backward through accelerated fixed-lag streams (a window tape and VJP with two anchor cotangents) does not exist
-    yet: refuse rather than differentiate the velocity-only problem."""
+    """The velocity-only backward entry points have no slot for the pre-anchor's cotangent: refuse an accelerated state
+    there rather than differentiate the velocity-only problem (its backward is the *_accel_vjp family)."""
     if taped and state.accel_weight:
-        raise ValueError(f"{what}: there is no backward through fixed-lag streams with an acceleration penalty "
-                         f"(accel_weight = {state.accel_weight}); only the forward and the flush run on them")
+        raise ValueError(f"{what}: this backward is the velocity-only one; fixed-lag streams with an acceleration penalty "
+                         f"(accel_weight = {state.accel_weight}) backpropagate through retarget_fixed_lag_accel_vjp, "
+                         "flush_fixed_lag_accel_vjp and the differentiable_*_fixed_lag_accel functions, with a tape from "
+                         "make_fixed_lag_tape(..., accel_weight=c)")
+
+
+def _check_tape_accel(state: FixedLagState, tape: Optional["FixedLagTape"]):
+    """`retarget_fixed_lag(tape=...)` records through the kernel of the state's c, so the tape must have been made for that
+    c: a velocity-only tape on an accelerated state is `_refuse_accel_backward`'s refusal, any other mismatch a ValueError."""
+    if tape is None or float(getattr(tape, "accel_weight", 0.0) or 0.0) == float(state.accel_weight):
+        return
+    if not getattr(tape, "accel_weight", 0.0):
+        _refuse_accel_backward(state, "retarget_fixed_lag(tape=...)")
+    raise ValueError(f"retarget_fixed_lag(tape=...): the tape was made for accel_weight = {tape.accel_weight}, the state "
+                     f"has {state.accel_weight}: record with make_fixed_lag_tape(..., accel_weight={state.accel_weight})")
 
 
 @dataclass
@@ -150,6 +164,8 @@ class FixedLagTape:
 
     qpos: "torch.Tensor"                 # [S, K, L+1, opt_dof] float32: each tick's window minimiser
     projected: Optional["torch.Tensor"]  # [S, K, len_proj] uint8: the committed flags each tick's solve started from, or None
+    # the acceleration penalty c of the state it records (`dexr_fixed_lag_step_accel_tape`); 0: a velocity-only state
+    accel_weight: float = 0.0
 
 
 @dataclass
@@ -835,10 +851,16 @@ class SeqRetargeting:
             prev_qpos=torch.zeros((num_streams, opt.opt_dof), dtype=torch.float32, device=dev) if accel else None,
             has_prev=torch.zeros((num_streams,), dtype=torch.int32, device=dev) if accel else None)
 
-    def make_fixed_lag_tape(self, num_streams: int, num_ticks: int, lag: int) -> FixedLagTape:
+    def make_fixed_lag_tape(self, num_streams: int, num_ticks: int, lag: int,
+                            accel_weight: Optional[float] = None) -> FixedLagTape:
         """Buffers for recording a `retarget_fixed_lag` call of K ticks on S streams of lag L (`tape=`), the input of
-        `retarget_fixed_lag_vjp`."""
+        `retarget_fixed_lag_vjp`.  `accel_weight` c: a tape for a state made with the same c (the layout is the same; the
+        recording runs `dexr_fixed_lag_step_accel_tape`), the input of `retarget_fixed_lag_accel_vjp`."""
         import torch
+
+        accel = 0.0 if accel_weight is None else float(accel_weight)
+        if not (accel == 0.0 or 0.0 < accel <= 3.0e38):
+            raise ValueError(f"accel_weight must be finite and >= 0, got {accel_weight}")
 
         opt = self.optimizer
         dev = torch.device("cuda", opt.engine().device)
@@ -846,11 +868,13 @@ class SeqRetargeting:
         S, K, L = int(num_streams), int(num_ticks), int(lag)
         return FixedLagTape(
             qpos=torch.empty((S, K, L + 1, opt.opt_dof), dtype=torch.float32, device=dev),
-            projected=torch.empty((S, K, len_proj), dtype=torch.uint8, device=dev) if len_proj else None)
+            projected=torch.empty((S, K, len_proj), dtype=torch.uint8, device=dev) if len_proj else None,
+            accel_weight=accel)
 
     def _fixed_lag_call(self, state: FixedLagState, K: int, fill, smooth_weight, stream, tape: Optional[FixedLagTape] = None):
         """One `dexr_fixed_lag_step` call on `state` with K ticks (`dexr_fixed_lag_step_tape` into `tape` when given,
-        `dexr_fixed_lag_step_accel` for an accelerated state); `fill(io, chk)` sets the per-call buffers."""
+        `dexr_fixed_lag_step_accel` for an accelerated state, `dexr_fixed_lag_step_accel_tape` for both); `fill(io, chk)`
+        sets the per-call buffers."""
         import torch
 
         opt = self.optimizer
@@ -884,6 +908,14 @@ class SeqRetargeting:
         io.workspace, io.workspace_bytes = ws.data_ptr(), nbytes
         s = stream if stream is not None else torch.cuda.current_stream(dev)
         p = opt.params(clip_init=True, lp_alpha=self.low_pass_alpha)
+        tp = None
+        if tape is not None:
+            tp = N.DexrFixedLagTape()
+            tp.qpos = chk(tape.qpos, (S, K, L + 1, n), torch.float32, "tape.qpos")
+            if len_proj:
+                if tape.projected is None:
+                    raise ValueError("DexPilot streams need tape.projected")
+                tp.projected = chk(tape.projected, (S, K, len_proj), torch.uint8, "tape.projected")
         if accel:
             acc = N.DexrFixedLagAccel()
             acc.accel_weight = accel
@@ -891,18 +923,17 @@ class SeqRetargeting:
                 raise ValueError("an accelerated fixed-lag state needs prev_qpos and has_prev")
             acc.prev_qpos = chk(state.prev_qpos, (S, n), torch.float32, "state.prev_qpos")
             acc.has_prev = chk(state.has_prev, (S,), torch.int32, "state.has_prev")
-            N.check(eng.lib.dexr_fixed_lag_step_accel(eng.handle, C.byref(p), C.byref(io), C.byref(acc), S, K,
-                                                      C.c_void_p(s.cuda_stream)), "dexr_fixed_lag_step_accel")
+            if tp is None:
+                N.check(eng.lib.dexr_fixed_lag_step_accel(eng.handle, C.byref(p), C.byref(io), C.byref(acc), S, K,
+                                                          C.c_void_p(s.cuda_stream)), "dexr_fixed_lag_step_accel")
+            else:
+                N.check(eng.lib.dexr_fixed_lag_step_accel_tape(eng.handle, C.byref(p), C.byref(io), C.byref(acc),
+                                                               C.byref(tp), S, K, C.c_void_p(s.cuda_stream)),
+                        "dexr_fixed_lag_step_accel_tape")
         elif tape is None:
             N.check(eng.lib.dexr_fixed_lag_step(eng.handle, C.byref(p), C.byref(io), S, K, C.c_void_p(s.cuda_stream)),
                     "dexr_fixed_lag_step")
         else:
-            tp = N.DexrFixedLagTape()
-            tp.qpos = chk(tape.qpos, (S, K, L + 1, n), torch.float32, "tape.qpos")
-            if len_proj:
-                if tape.projected is None:
-                    raise ValueError("DexPilot streams need tape.projected")
-                tp.projected = chk(tape.projected, (S, K, len_proj), torch.uint8, "tape.projected")
             N.check(eng.lib.dexr_fixed_lag_step_tape(eng.handle, C.byref(p), C.byref(io), C.byref(tp), S, K,
                                                      C.c_void_p(s.cuda_stream)), "dexr_fixed_lag_step_tape")
         ws.record_stream(s)
@@ -917,10 +948,12 @@ class SeqRetargeting:
         (STATUS_MISSING).  `state` (`make_fixed_lag_state`) is updated in place.  Returns (robot_qpos [S,K,dof] (scatter +
         mimic, no low-pass filter), qpos [S,K,opt_dof], status [S,K] int32), into `out` / `qpos_out` / `status_out` when
         given.  `tape` (`make_fixed_lag_tape(S, K, L)`): also record what `retarget_fixed_lag_vjp` needs; the outputs and
-        the state are the same bits either way.  Allocates its workspace on the device; nothing is synchronised."""
+        the state are the same bits either way.  An accelerated state records into a tape made with its own accel_weight
+        (for `retarget_fixed_lag_accel_vjp`); a tape whose c differs from the state's is refused (ValueError).  Allocates
+        its workspace on the device; nothing is synchronised."""
         import torch
 
-        _refuse_accel_backward(state, "retarget_fixed_lag(tape=...)", tape is not None)
+        _check_tape_accel(state, tape)
         opt = self.optimizer
         if keypoints.dim() != 4 or tuple(keypoints.shape[2:]) != (N.NUM_KEYPOINTS, 3):
             raise ValueError(f"keypoints must have shape [S,K,21,3], got {tuple(keypoints.shape)}")
@@ -969,11 +1002,12 @@ class SeqRetargeting:
         return rq, qpos, count
 
     def _fixed_lag_vjp_call(self, state0: FixedLagState, K: int, fill, flushed: bool, smooth_weight, grads: dict, stream,
-                            outputs: Optional[dict] = None):
+                            outputs: Optional[dict] = None, accel: bool = False):
         """One `dexr_fixed_lag_step_vjp` call: `state0` the state before the forward, `fill(io, chk, new)` the per-call
         buffers, `grads` the final state's cotangents (None = 0), `outputs` tensors to write the outputs into, by their
         dexr_fixed_lag_vjp_t names (the others are allocated).  Returns (grad_last_qpos, grad_window_keypoints,
-        grad_window_fixed_qpos or None, grad_window_qpos) of state0."""
+        grad_window_fixed_qpos or None, grad_window_qpos) of state0.  `accel`: `dexr_fixed_lag_step_accel_vjp` on the
+        accelerated state0 (grads may hold grad_prev_qpos_out, outputs grad_prev_qpos), grad_prev_qpos appended."""
         import torch
 
         opt = self.optimizer
@@ -1002,7 +1036,8 @@ class SeqRetargeting:
 
         outputs = outputs or {}
         unknown = set(outputs) - {"grad_keypoints", "grad_fixed_qpos", "grad_last_qpos", "grad_window_keypoints",
-                                  "grad_window_fixed_qpos", "grad_window_qpos", "status_out"}
+                                  "grad_window_fixed_qpos", "grad_window_qpos", "status_out"} - (
+                                      {"grad_prev_qpos"} if accel else set())
         if unknown:
             raise ValueError(f"outputs: unknown names {sorted(unknown)}")
 
@@ -1018,15 +1053,33 @@ class SeqRetargeting:
         g_wfix = new((S, L + 1, nf), "grad_window_fixed_qpos") if nf else None
         g_wq = new((S, L + 1, n), "grad_window_qpos")
         fill(io, chk, new)
-        nbytes = int(eng.lib.dexr_fixed_lag_vjp_workspace_bytes(eng.handle, S, L))
+        nbytes = int(eng.lib.dexr_fixed_lag_accel_vjp_workspace_bytes(eng.handle, S, L) if accel
+                     else eng.lib.dexr_fixed_lag_vjp_workspace_bytes(eng.handle, S, L))
         ws = torch.empty((max(nbytes, 4),), dtype=torch.uint8, device=dev)
         io.workspace, io.workspace_bytes = ws.data_ptr(), nbytes
         s = stream if stream is not None else torch.cuda.current_stream(dev)
         p = opt.params(clip_init=True, lp_alpha=self.low_pass_alpha)
-        N.check(eng.lib.dexr_fixed_lag_step_vjp(eng.handle, C.byref(p), C.byref(io), S, K, C.c_void_p(s.cuda_stream)),
-                "dexr_fixed_lag_step_vjp")
+        if not accel:
+            N.check(eng.lib.dexr_fixed_lag_step_vjp(eng.handle, C.byref(p), C.byref(io), S, K, C.c_void_p(s.cuda_stream)),
+                    "dexr_fixed_lag_step_vjp")
+            ws.record_stream(s)
+            return g_last, g_wkp, g_wfix, g_wq
+        if state0.prev_qpos is None or state0.has_prev is None:
+            raise ValueError("an accelerated fixed-lag state needs prev_qpos and has_prev")
+        acc = N.DexrFixedLagAccelVjp()
+        acc.accel_weight = float(state0.accel_weight)
+        acc.prev_qpos = chk(state0.prev_qpos, (S, n), torch.float32, "state0.prev_qpos")
+        acc.has_prev = chk(state0.has_prev, (S,), torch.int32, "state0.has_prev")
+        if grads.get("grad_prev_qpos_out") is not None:
+            acc.grad_prev_qpos_out = chk(grads["grad_prev_qpos_out"], (S, n), torch.float32, "grad_prev_qpos_out")
+        g_prev = outputs.get("grad_prev_qpos")
+        if g_prev is None:
+            g_prev = torch.empty((S, n), dtype=torch.float32, device=dev)
+        acc.grad_prev_qpos = chk(g_prev, (S, n), torch.float32, "outputs['grad_prev_qpos']")
+        N.check(eng.lib.dexr_fixed_lag_step_accel_vjp(eng.handle, C.byref(p), C.byref(io), C.byref(acc), S, K,
+                                                      C.c_void_p(s.cuda_stream)), "dexr_fixed_lag_step_accel_vjp")
         ws.record_stream(s)
-        return g_last, g_wkp, g_wfix, g_wq
+        return g_last, g_wkp, g_wfix, g_wq, g_prev
 
     def retarget_fixed_lag_vjp(self, keypoints, tape: FixedLagTape, state0: FixedLagState, *, fixed_qpos=None,
                                grad_qpos=None, grad_robot_qpos=None, grad_last_qpos_out=None, grad_window_qpos_out=None,
@@ -1046,6 +1099,16 @@ class SeqRetargeting:
         import torch
 
         _refuse_accel_backward(state0, "retarget_fixed_lag_vjp")
+        return self._retarget_fixed_lag_vjp(keypoints, tape, state0, fixed_qpos, grad_qpos, grad_robot_qpos,
+                                            grad_last_qpos_out, grad_window_qpos_out, grad_window_keypoints_out,
+                                            grad_window_fixed_qpos_out, smooth_weight, stream, outputs)
+
+    def _retarget_fixed_lag_vjp(self, keypoints, tape, state0, fixed_qpos, grad_qpos, grad_robot_qpos, grad_last_qpos_out,
+                                grad_window_qpos_out, grad_window_keypoints_out, grad_window_fixed_qpos_out, smooth_weight,
+                                stream, outputs, accel=False, grad_prev_qpos_out=None):
+        """retarget_fixed_lag_vjp, and retarget_fixed_lag_accel_vjp when `accel` (grad_prev_qpos appended)."""
+        import torch
+
         opt = self.optimizer
         if keypoints.dim() != 4 or tuple(keypoints.shape[2:]) != (N.NUM_KEYPOINTS, 3):
             raise ValueError(f"keypoints must have shape [S,K,21,3], got {tuple(keypoints.shape)}")
@@ -1075,10 +1138,9 @@ class SeqRetargeting:
 
         grads = dict(grad_last_qpos_out=grad_last_qpos_out, grad_window_qpos_out=grad_window_qpos_out,
                      grad_window_keypoints_out=grad_window_keypoints_out,
-                     grad_window_fixed_qpos_out=grad_window_fixed_qpos_out)
-        g_last, g_wkp, g_wfix, g_wq = self._fixed_lag_vjp_call(state0, K, fill, False, smooth_weight, grads, stream,
-                                                               outputs)
-        return res["kp"], res["fixed"], g_last, g_wkp, g_wfix, g_wq, res["status"]
+                     grad_window_fixed_qpos_out=grad_window_fixed_qpos_out, grad_prev_qpos_out=grad_prev_qpos_out)
+        r = self._fixed_lag_vjp_call(state0, K, fill, False, smooth_weight, grads, stream, outputs, accel)
+        return (res["kp"], res["fixed"], *r[:4], res["status"], *r[4:])
 
     def flush_fixed_lag_vjp(self, state0: FixedLagState, *, grad_qpos=None, grad_robot_qpos=None, grad_last_qpos_out=None,
                             grad_window_qpos_out=None, grad_window_keypoints_out=None, grad_window_fixed_qpos_out=None,
@@ -1090,6 +1152,15 @@ class SeqRetargeting:
         import torch
 
         _refuse_accel_backward(state0, "flush_fixed_lag_vjp")
+        return self._flush_fixed_lag_vjp(state0, grad_qpos, grad_robot_qpos, grad_last_qpos_out, grad_window_qpos_out,
+                                         grad_window_keypoints_out, grad_window_fixed_qpos_out, stream)
+
+    def _flush_fixed_lag_vjp(self, state0, grad_qpos, grad_robot_qpos, grad_last_qpos_out, grad_window_qpos_out,
+                             grad_window_keypoints_out, grad_window_fixed_qpos_out, stream, accel=False,
+                             grad_prev_qpos_out=None):
+        """flush_fixed_lag_vjp, and flush_fixed_lag_accel_vjp when `accel` (grad_prev_qpos appended)."""
+        import torch
+
         opt = self.optimizer
         S, L = int(state0.last_qpos.shape[0]), int(state0.lag)
         n, dof = opt.opt_dof, opt.robot.dof
@@ -1102,5 +1173,42 @@ class SeqRetargeting:
 
         grads = dict(grad_last_qpos_out=grad_last_qpos_out, grad_window_qpos_out=grad_window_qpos_out,
                      grad_window_keypoints_out=grad_window_keypoints_out,
-                     grad_window_fixed_qpos_out=grad_window_fixed_qpos_out)
-        return self._fixed_lag_vjp_call(state0, 0, fill, True, None, grads, stream)
+                     grad_window_fixed_qpos_out=grad_window_fixed_qpos_out, grad_prev_qpos_out=grad_prev_qpos_out)
+        return self._fixed_lag_vjp_call(state0, 0, fill, True, None, grads, stream, accel=accel)
+
+    @staticmethod
+    def _accel_state0(state0: FixedLagState, what: str, tape: Optional[FixedLagTape] = None):
+        if not state0.accel_weight:
+            raise ValueError(f"{what}: state0 has no acceleration penalty (accel_weight = 0): use "
+                             f"{what.replace('_accel', '')}")
+        if tape is not None and float(getattr(tape, "accel_weight", 0.0) or 0.0) != float(state0.accel_weight):
+            raise ValueError(f"{what}: the tape was recorded for accel_weight = {getattr(tape, 'accel_weight', 0.0)}, "
+                             f"state0 has {state0.accel_weight}")
+
+    def retarget_fixed_lag_accel_vjp(self, keypoints, tape: FixedLagTape, state0: FixedLagState, *, fixed_qpos=None,
+                                     grad_qpos=None, grad_robot_qpos=None, grad_last_qpos_out=None,
+                                     grad_prev_qpos_out=None, grad_window_qpos_out=None, grad_window_keypoints_out=None,
+                                     grad_window_fixed_qpos_out=None, smooth_weight=None, stream=None,
+                                     outputs: Optional[dict] = None):
+        """`retarget_fixed_lag_vjp` for a call on an accelerated state (`dexr_fixed_lag_step_accel_vjp`, one launch;
+        DESIGN.md 3.18): `tape` from `make_fixed_lag_tape(S, K, L, accel_weight=c)` with the state's c, `state0` the
+        accelerated state before the call.  Each differentiated window is the accel smoother's clip with the pre-anchor
+        triple of the forward; the reverse walk carries the cotangents of the last two committed frames.  Also takes
+        grad_prev_qpos_out [S,opt_dof], the cotangent of the final prev_qpos.  Returns retarget_fixed_lag_vjp's tuple with
+        grad_prev_qpos [S,opt_dof] (of state0.prev_qpos) appended; `outputs` may also name grad_prev_qpos.  The acceleration
+        weight and has_prev are not differentiated.  Nothing is synchronised."""
+        self._accel_state0(state0, "retarget_fixed_lag_accel_vjp", tape)
+        return self._retarget_fixed_lag_vjp(keypoints, tape, state0, fixed_qpos, grad_qpos, grad_robot_qpos,
+                                            grad_last_qpos_out, grad_window_qpos_out, grad_window_keypoints_out,
+                                            grad_window_fixed_qpos_out, smooth_weight, stream, outputs, True,
+                                            grad_prev_qpos_out)
+
+    def flush_fixed_lag_accel_vjp(self, state0: FixedLagState, *, grad_qpos=None, grad_robot_qpos=None,
+                                  grad_last_qpos_out=None, grad_prev_qpos_out=None, grad_window_qpos_out=None,
+                                  grad_window_keypoints_out=None, grad_window_fixed_qpos_out=None, stream=None):
+        """`flush_fixed_lag_vjp` for an accelerated state: also takes grad_prev_qpos_out and returns its tuple with
+        grad_prev_qpos (of state0.prev_qpos) appended."""
+        self._accel_state0(state0, "flush_fixed_lag_accel_vjp")
+        return self._flush_fixed_lag_vjp(state0, grad_qpos, grad_robot_qpos, grad_last_qpos_out, grad_window_qpos_out,
+                                         grad_window_keypoints_out, grad_window_fixed_qpos_out, stream, True,
+                                         grad_prev_qpos_out)

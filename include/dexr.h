@@ -643,7 +643,8 @@ int dexr_fixed_lag_step(const dexr_robot_t* robot, const dexr_params_t* params, 
  * are dexr_fixed_lag_step's.  DEXR_E_INVALID for any of dexr_fixed_lag_step's checks, a c that is <= 0 or non-finite,
  * prev_qpos or has_prev NULL while num_streams > 0, or io->workspace_bytes below
  * dexr_fixed_lag_accel_workspace_bytes(robot, num_streams, lag): the accel smoother's workspace for S (L+1) frames followed
- * by S (L+1) int32 status words.  There is no backward through accelerated streams yet.
+ * by S (L+1) int32 status words.  The backward is dexr_fixed_lag_step_accel_tape and dexr_fixed_lag_step_accel_vjp, after
+ * dexr_fixed_lag_step_vjp below.
  * ------------------------------------------------------------------------------------------- */
 typedef struct dexr_fixed_lag_accel {
   float accel_weight; /* c: finite, > 0 (c = 0 streams use dexr_fixed_lag_step)                                         */
@@ -753,6 +754,58 @@ size_t dexr_fixed_lag_vjp_sizeof(void);
 size_t dexr_fixed_lag_vjp_workspace_bytes(const dexr_robot_t* robot, int64_t num_streams, int32_t lag);
 int dexr_fixed_lag_step_vjp(const dexr_robot_t* robot, const dexr_params_t* params, const dexr_fixed_lag_vjp_t* io,
                             int64_t num_streams, int64_t num_ticks, void* cuda_stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * Backpropagation through fixed-lag smoothing with an acceleration penalty.
+ * dexr_fixed_lag_step_accel_tape is dexr_fixed_lag_step_accel that also records into `tape` as dexr_fixed_lag_step_tape
+ * does (same layout); its outputs and state, prev_qpos and has_prev included, are bit-identical to dexr_fixed_lag_step_accel's.
+ * Checks as dexr_fixed_lag_step_accel's plus dexr_fixed_lag_step_tape's tape check.
+ * dexr_fixed_lag_step_accel_vjp is dexr_fixed_lag_step_vjp for such a recorded call, `io` as there (io->smooth_weight w)
+ * and `acc` the acceleration weight c, the pre-anchor state before the call and the pre-anchor's cotangents.  With
+ * a_in = last_qpos, p_in = prev_qpos and hp_in = has_prev before the call, tick k's window has the anchor A_k, the
+ * pre-anchor P_k and the flag H_k:
+ *   c_k = 0: A_k = a_in, P_k = p_in, H_k = hp_in;   c_k = 1: X^{k-1}[0], a_in, 1;   c_k >= 2: X^{k-1}[0], X^{k-2}[0], 1.
+ * Window k is differentiated as dexr_smooth_sequences_packed_accel_vjp differentiates a clip anchored at clip(A_k), plus,
+ * when H_k = 1, the triple c |x_0 - 2 clip(A_k) + clip(P_k)|^2: 2c I more on block 0 of the Hessian, the anchor's cotangent
+ * (2w v_0) + (4c v_0 - 2c v_1 when the window has a second frame) + (4c v_0 when H_k = 1), summed in that order and all of
+ * it only where the clip passes A_k, and the pre-anchor's cotangent -2c v_0 where the clip passes P_k (0 when H_k = 0).
+ * The reverse walk carries two rows per stream: C1, the cotangent of X^k[0], and C2, that of X^{k-1}[0].  At the start C1
+ * is grad_last_qpos_out where the final last_qpos is X^{K-1}[0], and C2 is grad_prev_qpos_out where the final prev_qpos is
+ * X^{K-2}[0].  Slot 0 of an emitting window k gets its emitted row's cotangent + C1 (on the last tick, grad_last_qpos_out
+ * or grad_prev_qpos_out, whichever lands there).  After window k's VJP, with ga its anchor cotangent and gp its pre-anchor's:
+ *   c_k >= 2: C1 = C2 + ga, C2 = gp;   c_k = 1: C1 = C2 + ga, grad_last_qpos += gp;
+ *   c_k = 0:  grad_last_qpos += ga, grad_prev_qpos += gp.
+ * The final prev_qpos is the second-to-last committed frame, the incoming p_in and a_in counting as the two commits before
+ * the call; grad_prev_qpos_out goes to it: a flushed slot (summed after grad_last_qpos_out's place in the slot's order),
+ * X^{K-1}[0] (a flush of one frame), X^{K-2}[0] (C2), grad_last_qpos (written with it) or grad_prev_qpos (written with it).
+ * So the cotangent of a committed frame X^j[0] is its emitted row's + ((the pre-anchor cotangent of window j + 2) + (the
+ * anchor cotangent of window j + 1)), in that order, and a call split into chunks chained through grad_last_qpos /
+ * grad_prev_qpos gives the bits of one call.
+ * A NOT_PD window contributes zero and drops the slot cotangents that land on it, but no longer cuts the chain completely:
+ * the pre-anchor cotangent of the window after it (in C2) skips over it to X^{k-1}[0] -- correctly, as P_{k+1} does not
+ * pass through window k.  A non-finite point, anchor, pre-anchor (a non-finite prev_qpos with has_prev = 1 included) or
+ * cotangent makes the window's outputs NaN, which reaches earlier ticks through C1 and C2; other streams are untouched.
+ * Missing frames carry the chain; a flushed row's fixed-joint share starts its frame's sum.  Not differentiated: the
+ * DexPilot flags, w, c, has_prev and the warm start.  Everything else -- the outputs (grad_prev_qpos [S,n_var] too, written
+ * in full when non-NULL), status, layout, asynchrony -- is dexr_fixed_lag_step_vjp's.  DEXR_E_INVALID for any of
+ * dexr_fixed_lag_step_vjp's checks, a c that is <= 0 or non-finite, prev_qpos or has_prev NULL while num_streams > 0, or
+ * io->workspace_bytes below dexr_fixed_lag_accel_vjp_workspace_bytes(robot, num_streams, lag).
+ * ------------------------------------------------------------------------------------------- */
+typedef struct dexr_fixed_lag_accel_vjp {
+  float accel_weight;              /* c as given to the forward: finite, > 0                                             */
+  const float* prev_qpos;          /* [S,n_var] the pre-anchor before the call (raw)                                     */
+  const int32_t* has_prev;         /* [S] before the call                                                                */
+  const float* grad_prev_qpos_out; /* [S,n_var] cotangent of the final prev_qpos, or NULL (= 0)                          */
+  float* grad_prev_qpos;           /* [S,n_var] output: cotangent of the incoming prev_qpos, or NULL                     */
+} dexr_fixed_lag_accel_vjp_t;
+size_t dexr_fixed_lag_accel_vjp_sizeof(void);
+size_t dexr_fixed_lag_accel_vjp_workspace_bytes(const dexr_robot_t* robot, int64_t num_streams, int32_t lag);
+int dexr_fixed_lag_step_accel_tape(const dexr_robot_t* robot, const dexr_params_t* params, const dexr_fixed_lag_t* io,
+                                   const dexr_fixed_lag_accel_t* acc, const dexr_fixed_lag_tape_t* tape, int64_t num_streams,
+                                   int64_t num_ticks, void* cuda_stream);
+int dexr_fixed_lag_step_accel_vjp(const dexr_robot_t* robot, const dexr_params_t* params, const dexr_fixed_lag_vjp_t* io,
+                                  const dexr_fixed_lag_accel_vjp_t* acc, int64_t num_streams, int64_t num_ticks,
+                                  void* cuda_stream);
 
 #ifdef __cplusplus
 }
